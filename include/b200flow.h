@@ -171,14 +171,26 @@ typedef enum b2f_param_id {
                                      Brox: 0 = register-resident solver, one prepare + one solver launch per inner
                                      step, 1 = one launch per half sweep, 2 = shared-memory solver, 3 = all inner steps
                                      of a level in one cooperative launch.  All bit-identical.  */
-    B2F_ENGINE_AUX_PATH = 903     /* variant of the secondary kernels.  TV-L1 warp: 0 = tiled kernel (I1 window of a
+    B2F_ENGINE_AUX_PATH = 903,    /* variant of the secondary kernels.  TV-L1 warp: 0 = tiled kernel (I1 window of a
                                      64x32 tile staged in shared memory by TMA), 1 = tap-by-tap kernel (accumulation
                                      in the reference's order), 2 / 3 = separable kernel at 32 / 40 registers; 0, 2
                                      and 3 are bit-identical.  Farneback: fused iteration kernel
                                      at 0 = 128 registers (2 blocks / SM), 3 = 80, 4 = 64 registers, 5 = R1 gather
                                      with lanes on consecutive pixels, 6 = the simpler polynomial
                                      expansion and vertical-blur kernels.  All bit-identical.                                   */
+    /* TV-L1, read-only: B2F_ENGINE_ACTIVE_PATH + s is what the last calc ran on pyramid level s (0 = full size), an OR
+     * of b2f_tvl1_path flags; B2F_BAD_ARG for a level the last calc did not solve.  A shape whose tensor maps cannot be
+     * encoded falls back to the plain-load kernels; this says whether it did. */
+    B2F_ENGINE_ACTIVE_PATH = 1000
 } b2f_param_id;
+
+typedef enum b2f_tvl1_path {
+    B2F_TVL1_PATH_ITER_TMA = 1,       /* inner iterations: a persistent TMA-staged blocked kernel (kernel_path 0, 3-12) */
+    B2F_TVL1_PATH_ITER_BLOCKED = 2,   /* inner iterations: the blocked kernel with plain loads                          */
+    B2F_TVL1_PATH_ITER_UNFUSED = 4,   /* inner iterations: the unfused estimate_u / estimate_dual pair                  */
+    B2F_TVL1_PATH_WARP_TILED = 8,     /* warp: the tiled kernel, I1 window staged by TMA                                */
+    B2F_TVL1_PATH_WARP_UNTILED = 16   /* warp: the separable or tap-by-tap kernel                                       */
+} b2f_tvl1_path;
 
 /* cv::medianBlur for CV_32FC1, ksize 3 or 5, replicated border, not in place: the primitive behind
  * B2F_TVL1_MEDIAN_FILTERING (the reference's CPU path calls cv::medianBlur, modules/optflow/src/tvl1flow.cpp:1381-1382;

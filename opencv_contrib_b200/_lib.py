@@ -150,8 +150,10 @@ PARAM = {
     "brox": dict(alpha=300, gamma=301, scale_factor=302, inner_iterations=303, outer_iterations=304,
                  solver_iterations=305),
     "denselk": dict(win_width=400, win_height=401, max_level=402, iters=403, use_initial_flow=404),
-    "engine": dict(fused_iters=900, use_graph=901, kernel_path=902, aux_path=903),
+    "engine": dict(fused_iters=900, use_graph=901, kernel_path=902, aux_path=903, active_path=1000),
 }
+# b2f_tvl1_path flags (include/b200flow.h)
+TVL1_PATH = dict(iter_tma=1, iter_blocked=2, iter_unfused=4, warp_tiled=8, warp_untiled=16)
 
 _lib = None
 

@@ -691,6 +691,8 @@ private:
                          double scaledEps, dim3 grid, dim3 block, int nblocks, int rows, int cols);
     unsigned long long *iters_host_ = nullptr;  // pinned: EpsState::iters_total of the last device-loop solve
     bool device_loop_used_ = false;
+    // b2f_tvl1_path flags per solved level: of the last calc (B2F_ENGINE_ACTIVE_PATH) and of the captured graph
+    std::vector<int> level_paths_, graph_level_paths_;
 public:
     void refresh_stats() override {
         if (device_loop_used_ && iters_host_) stats.iterations_run = static_cast<int>(*iters_host_);
@@ -852,6 +854,7 @@ void Tvl1Engine::device_eps_loop(Ctx &c, int s, const Tvl1Planes &T, const Tvl1B
         Ctx b = c;
         b.stream = bs;
         const double npx = (double)rows * cols;
+        level_paths_[s] |= B2F_TVL1_PATH_ITER_TMA | B2F_TVL1_PATH_ITER_UNFUSED;
         tvl1_tma_launch_dev(b, CLS_ITER, tma_maps(s, 0), B, 0, rows, cols, k, &L_.eps->ia, num_sms_, knobs.kernel_path == 0);
         tvl1_tma_launch_dev(b, CLS_ITER, tma_maps(s, 1), B, 1, rows, cols, k, &L_.eps->ib, num_sms_, knobs.kernel_path == 0);
         B2F_LAUNCH(b, CLS_ITER, 48.0 * npx, k_tvl1_estimate_u, grid, block, 0, T, rows, cols, k, 1, L_.partials,
@@ -924,6 +927,7 @@ void Tvl1Engine::proc_one_scale(Ctx &c, int s, Plane &u3cur, bool allow_sync) {
     };
     auto run_blocked = [&](int count) {
         int done = 0;
+        if (count > 0) level_paths_[s] |= use_tma ? B2F_TVL1_PATH_ITER_TMA : B2F_TVL1_PATH_ITER_BLOCKED;
         while (done < count) {
             const int kk = tvl1_blocked_pick_k(knobs.fused_iters, count - done, rows, cols);
             if (use_tma && knobs.kernel_path == 5)  // paired-strip variant (two pixels per helper call)
@@ -969,11 +973,13 @@ void Tvl1Engine::proc_one_scale(Ctx &c, int s, Plane &u3cur, bool allow_sync) {
         // aux_path: 0 tiled (the default; levels smaller than one staged box take the separable kernel), 1 tap-by-tap in the
         // reference's order (62 registers, 4 blocks / SM), 2 separable at 32 registers (8 blocks / SM), 3 separable at 40
         // registers (6 blocks / SM; the default before the tiled kernel)
-        if (knobs.aux_path == 0 && warp_maps_ && cols >= WB_W && rows >= WB_H)  // I1 window staged by the copy engine
+        const bool tiled = (knobs.aux_path == 0 || knobs.aux_path == 4) && warp_maps_ && cols >= WB_W && rows >= WB_H;
+        level_paths_[s] |= tiled ? B2F_TVL1_PATH_WARP_TILED : B2F_TVL1_PATH_WARP_UNTILED;
+        if (tiled && knobs.aux_path == 0)  // I1 window staged by the copy engine
             B2F_LAUNCH(c, CLS_WARP, 32.0 * npx, k_tvl1_warp_tile<4>, dim3(div_up(cols, WT_W), div_up(rows, WT_H)),
                        dim3(WT_THREADS), 0, warp_maps_[s], lv.I0, lv.I1, T.u1, T.u2, T.I1wx, T.I1wy, T.grad, T.rho_c, rows,
                        cols);
-        else if (knobs.aux_path == 4 && warp_maps_ && cols >= WB_W && rows >= WB_H)  // same at 77 registers, 3 blocks / SM
+        else if (tiled)  // aux_path 4: the same at 77 registers, 3 blocks / SM
             B2F_LAUNCH(c, CLS_WARP, 32.0 * npx, k_tvl1_warp_tile<3>, dim3(div_up(cols, WT_W), div_up(rows, WT_H)),
                        dim3(WT_THREADS), 0, warp_maps_[s], lv.I0, lv.I1, T.u1, T.u2, T.I1wx, T.I1wy, T.grad, T.rho_c, rows,
                        cols);
@@ -1028,6 +1034,7 @@ void Tvl1Engine::proc_one_scale(Ctx &c, int s, Plane &u3cur, bool allow_sync) {
                 continue;
             }
             point_T_at(cur);
+            level_paths_[s] |= B2F_TVL1_PATH_ITER_UNFUSED;
             B2F_LAUNCH(c, CLS_ITER, 48.0 * npx, k_tvl1_estimate_u, grid, block, 0, T, rows, cols, k,
                        calcError ? 1 : 0, L_.partials, nullptr);
             if (calcError) {
@@ -1105,6 +1112,7 @@ int Tvl1Engine::calc(const b2f_image *I0, const b2f_image *I1, b2f_image *flow, 
     if (!c.ok()) return finish(c, s);
     stats.levels = L_.nscales;
     stats.iterations_run = 0;
+    level_paths_.assign(L_.nscales, 0);
 
     const ImageView v0{I0->data, I0->step, rows, cols, I0->type};
     const ImageView v1{I1->data, I1->step, rows, cols, I1->type};
@@ -1159,6 +1167,7 @@ int Tvl1Engine::calc(const b2f_image *I0, const b2f_image *I1, b2f_image *flow, 
                     graph_class_bytes_[i] = scratch.class_bytes[i] - stats.class_bytes[i];
                 }
                 graph_iterations_ = scratch.iterations_run;
+                graph_level_paths_ = level_paths_;
                 c.check(g.err);
                 if (c.ok()) {
                     graph_key_.rows = rows;
@@ -1181,6 +1190,7 @@ int Tvl1Engine::calc(const b2f_image *I0, const b2f_image *I1, b2f_image *flow, 
                 stats.class_bytes[i] += graph_class_bytes_[i];
             }
             stats.iterations_run = graph_iterations_;
+            level_paths_ = graph_level_paths_;
             if (dev_loop) {  // the true count lives on the device: fetch it behind the solve, read it in refresh_stats()
                 if (!iters_host_) c.check(cudaMallocHost(&iters_host_, sizeof(unsigned long long)));
                 if (c.ok())
@@ -1244,7 +1254,12 @@ int Tvl1Engine::get_param(int id, double *v) const {
         case B2F_TVL1_MEDIAN_FILTERING: *v = median_filtering; break;
         case B2F_TVL1_MEDIAN_PERIOD: *v = median_period; break;
         case B2F_TVL1_INITIAL_FLOW_SOURCE: *v = initial_flow_source; break;
-        default: return B2F_BAD_ARG;
+        default:
+            if (id >= B2F_ENGINE_ACTIVE_PATH && id - B2F_ENGINE_ACTIVE_PATH < (int)level_paths_.size()) {
+                *v = level_paths_[id - B2F_ENGINE_ACTIVE_PATH];
+                break;
+            }
+            return B2F_BAD_ARG;
     }
     return B2F_OK;
 }

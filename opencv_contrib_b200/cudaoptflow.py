@@ -205,6 +205,10 @@ class OpticalFlowDual_TVL1(DenseOpticalFlow):
     def _needs_initial_flow(self) -> bool:
         return bool(self.getUseInitialFlow()) and self.getInitialFlowSource() == 0
 
+    def getActivePath(self, level: int = 0) -> int:
+        """What the last calc ran on pyramid level `level`: an OR of _lib.TVL1_PATH flags (B2F_ENGINE_ACTIVE_PATH)."""
+        return int(self._get(PARAM["engine"]["active_path"] + level))
+
 
 _accessors(OpticalFlowDual_TVL1, "tvl1", {
     "tau": ("Tau", float), "lambda_": ("Lambda", float), "theta": ("Theta", float),

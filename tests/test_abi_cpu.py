@@ -76,9 +76,21 @@ def test_null_and_bad_arguments_fail_loudly(lib):
     assert lib.b2f_calc(h, None, None, None, None) == 1           # B2F_BAD_ARG
     assert lib.b2f_calc(h, C.byref(img), C.byref(img), C.byref(img), None) == 1
     assert lib.b2f_set_param(h, 12345, 1.0) == 1
+    v = C.c_double(-1.0)
+    active = _lib.PARAM["engine"]["active_path"]
+    assert lib.b2f_get_param(h, active, C.byref(v)) == 1 and v.value == -1.0  # no calc yet: no level to report
+    assert lib.b2f_set_param(h, active, 1.0) == 1                               # read-only
     assert b"B2F_BAD_ARG" in lib.b2f_status_string(1)
     lib.b2f_destroy(h)
     assert lib.b2f_tvl1_create(None, None) == 1
+
+
+def test_active_path_ids_match_header():
+    from opencv_contrib_b200 import _lib
+    src = open(os.path.join(ROOT, "include", "b200flow.h")).read()
+    flags = {m.group(1).lower(): int(m.group(2)) for m in re.finditer(r"B2F_TVL1_PATH_(\w+)\s*=\s*(\d+)", src)}
+    assert flags == _lib.TVL1_PATH
+    assert int(re.search(r"B2F_ENGINE_ACTIVE_PATH\s*=\s*(\d+)", src).group(1)) == _lib.PARAM["engine"]["active_path"]
 
 
 def test_header_is_plain_c99(tmp_path):
