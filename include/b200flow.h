@@ -170,7 +170,12 @@ typedef enum b2f_param_id {
                                      split-phase mbarriers.  All bit-identical; 0 is the default.
                                      Brox: 0 = register-resident solver, one prepare + one solver launch per inner
                                      step, 1 = one launch per half sweep, 2 = shared-memory solver, 3 = all inner steps
-                                     of a level in one cooperative launch.  All bit-identical.  */
+                                     of a level in one cooperative launch.  All bit-identical.
+                                     Farneback: 0 = auto (register-blocked quad kernel for winSize 13, the generic
+                                     kernel otherwise), 1 = the generic kernel for every winSize, 2 = the
+                                     register-blocked kernel with a per-pixel R1 gather, 3 = the persistent TMA
+                                     kernel on levels with at least 2 x n_SM 64x64 tiles (0 elsewhere).  All agree to
+                                     rounding; 3 is bit-identical to 0.  */
     B2F_ENGINE_AUX_PATH = 903,    /* variant of the secondary kernels.  TV-L1 warp: 0 = tiled kernel (I1 window of a
                                      64x32 tile staged in shared memory by TMA), 1 = tap-by-tap kernel (accumulation
                                      in the reference's order), 2 / 3 = separable kernel at 32 / 40 registers; 0, 2
@@ -178,11 +183,26 @@ typedef enum b2f_param_id {
                                      at 0 = 128 registers (2 blocks / SM), 3 = 80, 4 = 64 registers, 5 = R1 gather
                                      with lanes on consecutive pixels, 6 = the simpler polynomial
                                      expansion and vertical-blur kernels.  All bit-identical.                                   */
-    /* TV-L1, read-only: B2F_ENGINE_ACTIVE_PATH + s is what the last calc ran on pyramid level s (0 = full size), an OR
-     * of b2f_tvl1_path flags; B2F_BAD_ARG for a level the last calc did not solve.  A shape whose tensor maps cannot be
-     * encoded falls back to the plain-load kernels; this says whether it did. */
+    /* Read-only: B2F_ENGINE_ACTIVE_PATH + s is what the last calc ran on pyramid level s (0 = full size); B2F_BAD_ARG
+     * for a level the last calc did not solve.  TV-L1: an OR of b2f_tvl1_path flags.  A shape whose tensor maps cannot
+     * be encoded falls back to the plain-load kernels; this says whether it did.  Farneback: the b2f_farneback_path of
+     * the fused iteration kernel (0 with numIters = 0).  kernel_path 3 falls back to the fast kernel on levels with
+     * fewer than 2 x n_SM 64x64 tiles or whose tensor maps cannot be encoded; this says whether it did. */
     B2F_ENGINE_ACTIVE_PATH = 1000
 } b2f_param_id;
+
+/* Fused Farneback iteration kernels.  The box and gaussian windows share a value. */
+typedef enum b2f_farneback_path {
+    B2F_FARN_PATH_TMA = 1,             /* persistent kernel, M tiles staged by TMA (kernel_path 3)                  */
+    B2F_FARN_PATH_QUAD = 2,            /* register-blocked, quad R1 gather, 256 threads, 128 registers (the gaussian
+                                          window always runs this one)                                              */
+    B2F_FARN_PATH_QUAD_WIDE = 3,       /* the same at 512 threads: box levels with at most n_SM 64x32 tiles          */
+    B2F_FARN_PATH_QUAD_R80 = 4,        /* 256 threads at 80 registers (aux_path 3)                                   */
+    B2F_FARN_PATH_QUAD_R64 = 5,        /* 256 threads at 64 registers (aux_path 4)                                   */
+    B2F_FARN_PATH_QUAD_TRANSPOSED = 6, /* 256 threads, lanes on consecutive pixels in the R1 gather (aux_path 5)     */
+    B2F_FARN_PATH_FAST = 7,            /* register-blocked, per-pixel R1 gather (kernel_path 2)                      */
+    B2F_FARN_PATH_GENERIC = 8          /* k_farn_iter: any winSize other than 13, or kernel_path 1                   */
+} b2f_farneback_path;
 
 typedef enum b2f_tvl1_path {
     B2F_TVL1_PATH_ITER_TMA = 1,       /* inner iterations: a persistent TMA-staged blocked kernel (kernel_path 0, 3-12) */

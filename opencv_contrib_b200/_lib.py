@@ -154,6 +154,8 @@ PARAM = {
 }
 # b2f_tvl1_path flags (include/b200flow.h)
 TVL1_PATH = dict(iter_tma=1, iter_blocked=2, iter_unfused=4, warp_tiled=8, warp_untiled=16)
+# b2f_farneback_path values (include/b200flow.h)
+FARN_PATH = dict(tma=1, quad=2, quad_wide=3, quad_r80=4, quad_r64=5, quad_transposed=6, fast=7, generic=8)
 
 _lib = None
 

@@ -1194,6 +1194,9 @@ private:
         EngineKnobs knobs;
         void *base = nullptr;
     } graph_key_;
+    // b2f_farneback_path of the iteration kernel per solved level: of the last calc (B2F_ENGINE_ACTIVE_PATH) and of
+    // the captured graph
+    std::vector<int> level_paths_, graph_level_paths_;
     void solve(Ctx &c);
 
     size_t layout(int rows, int cols, bool counting, Layout &L, std::vector<float> &tabs);
@@ -1273,7 +1276,9 @@ size_t FarnebackEngine::layout(int rows, int cols, bool counting, Layout &L, std
         L.vbuf[1] = A.plane(2 * max_lrows, cols);
     }
     for (int i = 0; i < 2; ++i) {
-        Plane r = A.plane(5 * rows, cols), m = A.plane(5 * rows, cols);
+        // R gets one spare row: the quad / spread gathers point a pixel without a bilinear cell at (0, 0) and still
+        // load its row below, which on a one-row level lies one row past plane 4 (the loaded values are discarded)
+        Plane r = A.plane(5 * rows + 1, cols), m = A.plane(5 * rows, cols);
         L.R[i] = Stack5{r.p, r.pitch, rows};
         L.M[i] = Stack5{m.p, m.pitch, rows};
     }
@@ -1346,6 +1351,7 @@ int FarnebackEngine::calc(const b2f_image *I0, const b2f_image *I1, b2f_image *f
     const int top = static_cast<int>(L.levels.size()) - 1;
     stats.levels = top + 1;
     stats.iterations_run = 0;
+    level_paths_.assign(top + 1, 0);
 
     const ImageView v0{I0->data, I0->step, rows, cols, I0->type};
     const ImageView v1{I1->data, I1->step, rows, cols, I1->type};
@@ -1370,9 +1376,11 @@ int FarnebackEngine::calc(const b2f_image *I0, const b2f_image *I1, b2f_image *f
                 graph_key_.P = P;
                 graph_key_.knobs = knobs;
                 graph_key_.base = L.frames[0].p;
+                graph_level_paths_ = level_paths_;
             }
         }
         graph_.replay(*this, c, s);
+        if (c.ok()) level_paths_ = graph_level_paths_;
     } else {
         solve(c);
     }
@@ -1482,6 +1490,19 @@ void FarnebackEngine::solve(Ctx &c) {
             use_tma = tma_encode_2d_f32(&mapA, Ma.p, (uint64_t)w, 5ull * h, pitch_b, TB_W, TB_H) &&
                       tma_encode_2d_f32(&mapB, Mb.p, (uint64_t)w, 5ull * h, pitch_b, TB_W, TB_H);
         }
+        {  // the kernel the loop below launches (same branch order), reported through B2F_ENGINE_ACTIVE_PATH + k
+            const bool quad = knobs.kernel_path != 2;
+            int path = B2F_FARN_PATH_GENERIC;
+            if (use_tma) path = B2F_FARN_PATH_TMA;
+            else if (fast6 && !quad) path = B2F_FARN_PATH_FAST;
+            else if (fast6 && gauss) path = B2F_FARN_PATH_QUAD;
+            else if (fast6 && wide_blocks) path = B2F_FARN_PATH_QUAD_WIDE;
+            else if (fast6 && knobs.aux_path == 3) path = B2F_FARN_PATH_QUAD_R80;
+            else if (fast6 && knobs.aux_path == 5) path = B2F_FARN_PATH_QUAD_TRANSPOSED;
+            else if (fast6 && knobs.aux_path == 4) path = B2F_FARN_PATH_QUAD_R64;
+            else if (fast6) path = B2F_FARN_PATH_QUAD;
+            level_paths_[k] = P.num_iters > 0 ? path : 0;
+        }
         bool a_is_input = true;
         for (int i = 0; i < P.num_iters; ++i) {
             const int upd = i < P.num_iters - 1;  // farneback.cpp:468-470
@@ -1566,7 +1587,12 @@ int FarnebackEngine::get_param(int id, double *v) const {
         case B2F_FARN_POLY_N: *v = P.poly_n; break;
         case B2F_FARN_POLY_SIGMA: *v = P.poly_sigma; break;
         case B2F_FARN_FLAGS: *v = P.flags; break;
-        default: return B2F_BAD_ARG;
+        default:
+            if (id >= B2F_ENGINE_ACTIVE_PATH && id - B2F_ENGINE_ACTIVE_PATH < (int)level_paths_.size()) {
+                *v = level_paths_[id - B2F_ENGINE_ACTIVE_PATH];
+                break;
+            }
+            return B2F_BAD_ARG;
     }
     return B2F_OK;
 }

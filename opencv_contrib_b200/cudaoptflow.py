@@ -226,6 +226,11 @@ class FarnebackOpticalFlow(DenseOpticalFlow):
     def _needs_initial_flow(self) -> bool:
         return (int(self.getFlags()) & OPTFLOW_USE_INITIAL_FLOW) != 0
 
+    def getActivePath(self, level: int = 0) -> int:
+        """The fused iteration kernel the last calc ran on pyramid level `level`: a _lib.FARN_PATH value
+        (B2F_ENGINE_ACTIVE_PATH)."""
+        return int(self._get(PARAM["engine"]["active_path"] + level))
+
 
 _accessors(FarnebackOpticalFlow, "farneback", {
     "num_levels": ("NumLevels", int), "pyr_scale": ("PyrScale", float), "fast_pyramids": ("FastPyramids", bool),

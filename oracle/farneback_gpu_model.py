@@ -65,7 +65,7 @@ def prepare_gaussian(n: int, sigma: float):
 
 
 def poly_exp(src: np.ndarray, n: int, sigma: float) -> np.ndarray:
-    """polynomialExpansion<polyN> (CO/src/cuda/farneback.cu:66-119).  Returns R (5, H, W)."""
+    """polynomialExpansion<polyN> (CO/src/cuda/farneback.cu:66-119).  Returns R (5, H, W) in src's dtype."""
     g, xg, xxg, ig11, ig03, ig33, ig55 = prepare_gaussian(n, sigma)
     H, W = src.shape
     ys = np.arange(H)
@@ -96,54 +96,57 @@ def poly_exp(src: np.ndarray, n: int, sigma: float) -> np.ndarray:
         b3 = b3 + (col(r1, k) + col(r1, -k)) * g[k]
         b6 = b6 + (col(r1, k) - col(r1, -k)) * xg[k]
         b5 = b5 + (col(r2, k) + col(r2, -k)) * g[k]
-    R = np.stack([b3 * ig11, b2 * ig11, b1 * ig03 + b5 * ig33, b1 * ig03 + b4 * ig33, b6 * ig55]).astype(F)
+    R = np.stack([b3 * ig11, b2 * ig11, b1 * ig03 + b5 * ig33, b1 * ig03 + b4 * ig33, b6 * ig55]).astype(src.dtype)
     return R
 
 
 def update_matrices(fx_, fy_, R0, R1) -> np.ndarray:
-    """updateMatrices (CO/src/cuda/farneback.cu:156-241).  Returns M (5, H, W)."""
+    """updateMatrices (CO/src/cuda/farneback.cu:156-241).  Returns M (5, H, W) in the flow's dtype."""
+    D = fx_.dtype.type
     H, W = fx_.shape
     ys, xs = np.mgrid[0:H, 0:W]
     dx, dy = fx_, fy_
-    fx = xs.astype(F) + dx
-    fy = ys.astype(F) + dy
+    fx = xs.astype(D) + dx
+    fy = ys.astype(D) + dy
     x1 = np.floor(fx).astype(np.int64)
     y1 = np.floor(fy).astype(np.int64)
-    fx = (fx - x1.astype(F)).astype(F)
-    fy = (fy - y1.astype(F)).astype(F)
+    fx = (fx - x1.astype(D)).astype(D)
+    fy = (fy - y1.astype(D)).astype(D)
     inb = (x1 >= 0) & (y1 >= 0) & (x1 < W - 1) & (y1 < H - 1)
     x1c = np.clip(x1, 0, W - 2)
     y1c = np.clip(y1, 0, H - 2)
-    a00 = (F(1) - fx) * (F(1) - fy)
-    a01 = fx * (F(1) - fy)
-    a10 = (F(1) - fx) * fy
+    a00 = (D(1) - fx) * (D(1) - fy)
+    a01 = fx * (D(1) - fy)
+    a10 = (D(1) - fx) * fy
     a11 = fx * fy
 
     def gather(P):
-        return (a00 * P[y1c, x1c] + a01 * P[y1c, x1c + 1] + a10 * P[y1c + 1, x1c] + a11 * P[y1c + 1, x1c + 1]).astype(F)
+        return (a00 * P[y1c, x1c] + a01 * P[y1c, x1c + 1] + a10 * P[y1c + 1, x1c] + a11 * P[y1c + 1, x1c + 1]).astype(D)
 
-    r2 = np.where(inb, gather(R1[0]), F(0)).astype(F)
-    r3 = np.where(inb, gather(R1[1]), F(0)).astype(F)
-    r4 = np.where(inb, (R0[2] + gather(R1[2])) * F(0.5), R0[2]).astype(F)
-    r5 = np.where(inb, (R0[3] + gather(R1[3])) * F(0.5), R0[3]).astype(F)
-    r6 = np.where(inb, (R0[4] + gather(R1[4])) * F(0.25), R0[4] * F(0.5)).astype(F)
-    r2 = (R0[0] - r2) * F(0.5)
-    r3 = (R0[1] - r3) * F(0.5)
+    r2 = np.where(inb, gather(R1[0]), D(0)).astype(D)
+    r3 = np.where(inb, gather(R1[1]), D(0)).astype(D)
+    r4 = np.where(inb, (R0[2] + gather(R1[2])) * D(0.5), R0[2]).astype(D)
+    r5 = np.where(inb, (R0[3] + gather(R1[3])) * D(0.5), R0[3]).astype(D)
+    r6 = np.where(inb, (R0[4] + gather(R1[4])) * D(0.25), R0[4] * D(0.5)).astype(D)
+    r2 = (R0[0] - r2) * D(0.5)
+    r3 = (R0[1] - r3) * D(0.5)
     r2 = r2 + r4 * dy + r6 * dx
     r3 = r3 + r6 * dy + r5 * dx
     bs = 5
-    scale = (BORDER[np.minimum(xs, bs)] * BORDER[np.minimum(ys, bs)] *
-             BORDER[np.minimum(W - xs - 1, bs)] * BORDER[np.minimum(H - ys - 1, bs)]).astype(F)
+    B = BORDER.astype(D)
+    scale = (B[np.minimum(xs, bs)] * B[np.minimum(ys, bs)] *
+             B[np.minimum(W - xs - 1, bs)] * B[np.minimum(H - ys - 1, bs)]).astype(D)
     r2, r3, r4, r5, r6 = r2 * scale, r3 * scale, r4 * scale, r5 * scale, r6 * scale
     return np.stack([r4 * r4 + r6 * r6, (r4 + r5) * r6, r5 * r5 + r6 * r6, r4 * r2 + r6 * r3,
-                     r6 * r2 + r5 * r3]).astype(F)
+                     r6 * r2 + r5 * r3]).astype(D)
 
 
 def update_flow(M):
     """updateFlow (CO/src/cuda/farneback.cu:267-286)."""
+    D = M.dtype.type
     g11, g12, g22, h1, h2 = M
-    det_inv = F(1.0) / (g11 * g22 - g12 * g12 + F(1e-3))
-    return ((g11 * h2 - g12 * h1) * det_inv).astype(F), ((g22 * h1 - g12 * h2) * det_inv).astype(F)
+    det_inv = D(1.0) / (g11 * g22 - g12 * g12 + D(F(1e-3)))
+    return ((g11 * h2 - g12 * h1) * det_inv).astype(D), ((g22 * h1 - g12 * h2) * det_inv).astype(D)
 
 
 def _sep_filter(P, taps, border):
@@ -167,7 +170,7 @@ def _sep_filter(P, taps, border):
     res = row * taps[0]
     for i in range(1, k + 1):
         res = res + (row[..., :, rx(xs - i)] + row[..., :, rx(xs + i)]) * taps[i]
-    return res.astype(F)
+    return res.astype(P.dtype)
 
 
 def box_filter5(M, ksize_half):
@@ -181,7 +184,7 @@ def box_filter5(M, ksize_half):
     for i in range(1, ksize_half + 1):
         res = res + (row[:, :, np.clip(xs - i, 0, W - 1)] + row[:, :, np.clip(xs + i, 0, W - 1)])
     inv = F(1.0 / ((1 + 2 * ksize_half) * (1 + 2 * ksize_half)))
-    return (res * inv).astype(F)
+    return (res * inv).astype(M.dtype)
 
 
 def gaussian_kernel_half(ksize, sigma):
@@ -196,13 +199,38 @@ def pyr_down(src):
     return cv2.pyrDown(src)
 
 
-def calc(I0, I1, P: FarnebackParams | None = None, init_flow=None, stages=None):
-    """FarnebackOpticalFlowImpl::calc/calcImpl (CO/src/farneback.cpp:167-482)."""
+def level_sizes(H: int, W: int, P: FarnebackParams):
+    """(rows, cols) of pyramid levels 0 (full size) .. top, as calc() builds them."""
+    scale, cropped = 1.0, 0
+    while cropped < P.numLevels:
+        scale *= P.pyrScale
+        if W * scale < MIN_SIZE or H * scale < MIN_SIZE:
+            break
+        cropped += 1
+    sizes = [(H, W)]
+    for k in range(1, cropped + 1):
+        if P.fastPyramids:
+            sizes.append(((sizes[-1][0] + 1) // 2, (sizes[-1][1] + 1) // 2))
+        else:
+            s = 1.0
+            for _ in range(k):
+                s *= P.pyrScale
+            sizes.append((cv_round(H * s), cv_round(W * s)))
+    return sizes
+
+
+def calc(I0, I1, P: FarnebackParams | None = None, init_flow=None, stages=None, precision="f32"):
+    """FarnebackOpticalFlowImpl::calc/calcImpl (CO/src/farneback.cpp:167-482).
+
+    precision "f32" restates the kernels' float arithmetic; "f64" runs every operation in double (the constant tables
+    -- polynomial-expansion and window kernels, border weights, resize scales -- keep the float values both use), a
+    yardstick for how far float rounding alone moves the flow."""
+    D = {"f32": F, "f64": np.float64}[precision]
     P = P or FarnebackParams()
     assert P.polyN in (5, 7)
     assert (not P.fastPyramids) or abs(P.pyrScale - 0.5) < 1e-6
     H, W = I0.shape
-    frames = [I0.astype(F), I1.astype(F)]   # convertTo(CV_32F), no scaling (:342-345)
+    frames = [I0.astype(D), I1.astype(D)]   # convertTo(CV_32F), no scaling (:342-345)
     scale = 1.0
     cropped = 0
     while cropped < P.numLevels:
@@ -228,14 +256,14 @@ def calc(I0, I1, P: FarnebackParams | None = None, init_flow=None, stages=None):
             h, w = pyr[0][k].shape
         if prev is None:
             if P.flags & OPTFLOW_USE_INITIAL_FLOW:
-                fx = resize_linear(init_flow[..., 0].astype(F), dsize=(h, w)) * F(scale)
-                fy = resize_linear(init_flow[..., 1].astype(F), dsize=(h, w)) * F(scale)
+                fx = resize_linear(init_flow[..., 0].astype(D), dsize=(h, w), dtype=D) * F(scale)
+                fy = resize_linear(init_flow[..., 1].astype(D), dsize=(h, w), dtype=D) * F(scale)
             else:
-                fx = np.zeros((h, w), F)
-                fy = np.zeros((h, w), F)
+                fx = np.zeros((h, w), D)
+                fy = np.zeros((h, w), D)
         else:
-            fx = resize_linear(prev[0], dsize=(h, w)) * F(1.0 / P.pyrScale)
-            fy = resize_linear(prev[1], dsize=(h, w)) * F(1.0 / P.pyrScale)
+            fx = resize_linear(prev[0], dsize=(h, w), dtype=D) * F(1.0 / P.pyrScale)
+            fy = resize_linear(prev[1], dsize=(h, w), dtype=D) * F(1.0 / P.pyrScale)
         R = []
         for i in range(2):
             if P.fastPyramids:
@@ -243,7 +271,7 @@ def calc(I0, I1, P: FarnebackParams | None = None, init_flow=None, stages=None):
             else:
                 g = gaussian_kernel_half(smooth, sigma)
                 blurred = _sep_filter(frames[i], g, "reflect101")
-                lvl = resize_linear(blurred, dsize=(h, w))
+                lvl = resize_linear(blurred, dsize=(h, w), dtype=D)
             R.append(poly_exp(lvl, P.polyN, P.polySigma))
             if stages is not None:
                 stages.setdefault("level_image", {})[(k, i)] = lvl

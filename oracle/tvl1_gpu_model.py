@@ -48,9 +48,10 @@ def level_sizes(h: int, w: int, nscales: int, scaleStep: float):
     return sizes, nscales
 
 
-def resize_linear(src: np.ndarray, dsize=None, fx: float = 0.0, fy: float = 0.0) -> np.ndarray:
+def resize_linear(src: np.ndarray, dsize=None, fx: float = 0.0, fy: float = 0.0, dtype=F) -> np.ndarray:
     """cv::cuda::resize INTER_LINEAR, float C1 (CW/src/resize.cpp:57-106, CW/src/cuda/resize.cu:234-269).
-    src = dst*scale (no half-pixel centre), scale = float(1/f), right/bottom taps clamped."""
+    src = dst*scale (no half-pixel centre), scale = float(1/f), right/bottom taps clamped.  dtype: the arithmetic
+    (np.float64 gives a double-precision yardstick; the scale stays the float value the kernel uses)."""
     H, W = src.shape
     if dsize is None:
         dw, dh = cv_round(W * fx), cv_round(H * fy)
@@ -59,23 +60,24 @@ def resize_linear(src: np.ndarray, dsize=None, fx: float = 0.0, fy: float = 0.0)
         fx, fy = dw / W, dh / H
     if (dh, dw) == (H, W):
         return src.copy()
-    sx, sy = F(1.0 / fx), F(1.0 / fy)
-    src_x = np.arange(dw, dtype=F) * sx
-    src_y = np.arange(dh, dtype=F) * sy
+    D = dtype
+    sx, sy = D(F(1.0 / fx)), D(F(1.0 / fy))
+    src_x = np.arange(dw, dtype=D) * sx
+    src_y = np.arange(dh, dtype=D) * sy
     x1 = np.floor(src_x).astype(np.int64)
     y1 = np.floor(src_y).astype(np.int64)
     x2, y2 = x1 + 1, y1 + 1
     x2r, y2r = np.minimum(x2, W - 1), np.minimum(y2, H - 1)
-    wx2 = (x2.astype(F) - src_x)[None, :]
-    wx1 = (src_x - x1.astype(F))[None, :]
-    wy2 = (y2.astype(F) - src_y)[:, None]
-    wy1 = (src_y - y1.astype(F))[:, None]
-    out = np.zeros((dh, dw), F)
+    wx2 = (x2.astype(D) - src_x)[None, :]
+    wx1 = (src_x - x1.astype(D))[None, :]
+    wy2 = (y2.astype(D) - src_y)[:, None]
+    wy1 = (src_y - y1.astype(D))[:, None]
+    out = np.zeros((dh, dw), D)
     out = out + src[np.ix_(y1, x1)] * (wx2 * wy2)
     out = out + src[np.ix_(y1, x2r)] * (wx1 * wy2)
     out = out + src[np.ix_(y2r, x1)] * (wx2 * wy1)
     out = out + src[np.ix_(y2r, x2r)] * (wx1 * wy1)
-    return out.astype(F)
+    return out.astype(D)
 
 
 def centered_gradient(src):

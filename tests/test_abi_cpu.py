@@ -90,6 +90,9 @@ def test_active_path_ids_match_header():
     src = open(os.path.join(ROOT, "include", "b200flow.h")).read()
     flags = {m.group(1).lower(): int(m.group(2)) for m in re.finditer(r"B2F_TVL1_PATH_(\w+)\s*=\s*(\d+)", src)}
     assert flags == _lib.TVL1_PATH
+    farn = {m.group(1).lower(): int(m.group(2)) for m in re.finditer(r"B2F_FARN_PATH_(\w+)\s*=\s*(\d+)", src)}
+    assert farn == _lib.FARN_PATH
+    assert len(set(farn.values())) == len(farn) and 0 not in farn.values()  # 0 means "no iteration ran"
     assert int(re.search(r"B2F_ENGINE_ACTIVE_PATH\s*=\s*(\d+)", src).group(1)) == _lib.PARAM["engine"]["active_path"]
 
 

@@ -153,16 +153,22 @@ def test_persistent_tma_iteration_kernel_bit_identical(cuda_device, flags):
 
 def test_iteration_kernel_register_variants_bit_identical(cuda_device):
     """aux_path picks the register cap (= resident blocks per SM) of the fused iteration kernel: 0 -> 128 registers
-    (default), 3 -> 80, 4 -> 64.  Same arithmetic -> same bits."""
+    (default), 3 -> 80, 4 -> 64, 5 -> the lane-transposed R1 gather.  They run on levels with more than n_SM 64x32 tiles
+    (smaller levels take the 512-thread kernel), so level 0 is sized from the SM count.  Same arithmetic -> same bits."""
     import torch
     import opencv_contrib_b200 as ocb
-    I0, I1, _ = synth.make_pair(270, 480, seed=13, kind="smooth")
+    from opencv_contrib_b200._lib import FARN_PATH
+    n_sm = torch.cuda.get_device_properties(cuda_device).multi_processor_count
+    h, w = 32 * (n_sm // 15 + 2) - 5, 960 - 27   # 15 x (n_SM / 15 + 2) > n_SM tiles at level 0, about a quarter at level 1
+    I0, I1, _ = synth.make_pair(h, w, seed=13, kind="smooth")
     d0, d1 = torch.from_numpy(I0).to(cuda_device), torch.from_numpy(I1).to(cuda_device)
     outs = []
-    for aux in (0, 3, 4, 5):
+    for aux, path in ((0, "quad"), (3, "quad_r80"), (4, "quad_r64"), (5, "quad_transposed")):
         alg = ocb.FarnebackOpticalFlow_create()
         alg.setEngineOption("aux_path", aux)
         outs.append(alg.calc(d0, d1).cpu().numpy())
+        levels = alg.getStats()["levels"]
+        assert [alg.getActivePath(k) for k in range(levels)] == [FARN_PATH[path]] + [FARN_PATH["quad_wide"]] * (levels - 1)
     for o in outs[1:]:
         assert np.array_equal(outs[0], o)
 

@@ -32,6 +32,33 @@ for name, alg, a, b in [
     torch.cuda.synchronize()
     print(name, "ok", float(fl.abs().mean()), flush=True)
 fl = fl.contiguous()
+# Farneback iteration-kernel variants: (name, size, create() arguments, kernel_path, aux_path).  983 x 1053 has more than
+# 2 x 132 64x64 tiles, so kernel_path 3 runs the persistent TMA kernel there; the other sizes have more than 132 64x32
+# tiles at level 0 where the aux variants need it.
+for name, (h, w), kw, kp, aux in [
+        ("farneback-generic", (141, 203), dict(numLevels=2, numIters=2), 1, 0),
+        ("farneback-pixel-gather", (141, 203), dict(numLevels=2, numIters=2, flags=256), 2, 0),
+        ("farneback-tma", (983, 1053), dict(numLevels=0, numIters=2), 3, 0),
+        ("farneback-aux3", (315, 933), dict(numLevels=1, numIters=2), 0, 3),
+        ("farneback-aux4", (315, 933), dict(numLevels=1, numIters=2), 0, 4),
+        ("farneback-aux5", (315, 933), dict(numLevels=1, numIters=2), 0, 5),
+        ("farneback-win1", (141, 203), dict(numLevels=1, numIters=2, winSize=1), 0, 0),
+        ("farneback-win31", (141, 203), dict(numLevels=1, numIters=2, winSize=31, flags=256), 0, 0),
+        ("farneback-1x37", (1, 37), dict(numLevels=0, numIters=3), 0, 0),
+        ("farneback-37x1", (37, 1), dict(numLevels=0, numIters=3, flags=256), 0, 0)]:
+    if len(sys.argv) > 1 and not any(name.startswith(a) for a in sys.argv[1:]):
+        continue
+    J0, J1, _ = synth.make_pair(max(h, 16), max(w, 16), seed=5, kind="smooth")
+    j0 = torch.from_numpy(np.ascontiguousarray(J0[:h, :w])).to(dev)
+    j1 = torch.from_numpy(np.ascontiguousarray(J1[:h, :w])).to(dev)
+    alg = ocb.FarnebackOpticalFlow_create(**kw)
+    alg.setEngineOption("kernel_path", kp)
+    alg.setEngineOption("aux_path", aux)
+    alg.setEngineOption("use_graph", 0)
+    ff = alg.calc(j0, j1)
+    torch.cuda.synchronize()
+    print(name, "ok", float(ff.abs().mean()), "active path", [alg.getActivePath(k) for k in range(alg.getStats()["levels"])],
+          flush=True)
 mid = ocb.interpolateFrames(f0, f1, fl[..., 0].contiguous(), fl[..., 1].contiguous(), -fl[..., 0].contiguous(),
                             -fl[..., 1].contiguous(), 0.3)
 mid2 = ocb.interpolateFrames(f0, f1, fl[..., 0].contiguous(), fl[..., 1].contiguous(), -fl[..., 0].contiguous(),
