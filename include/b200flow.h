@@ -182,12 +182,21 @@ typedef enum b2f_param_id {
                                      and 3 are bit-identical.  Farneback: fused iteration kernel
                                      at 0 = 128 registers (2 blocks / SM), 3 = 80, 4 = 64 registers, 5 = R1 gather
                                      with lanes on consecutive pixels, 6 = the simpler polynomial
-                                     expansion and vertical-blur kernels.  All bit-identical.                                   */
+                                     expansion and vertical-blur kernels.  All bit-identical.
+                                     Brox (a test knob): 0 = the data term's reciprocal square root by rsqrtf, as the
+                                     reference computes it (the default; up to 2 ulp, bits not specified by CUDA), 1 =
+                                     correctly rounded (__frsqrt_rn), so that a float model can match the engine bit
+                                     for bit.  Nothing else depends on it.                                             */
     /* Read-only: B2F_ENGINE_ACTIVE_PATH + s is what the last calc ran on pyramid level s (0 = full size); B2F_BAD_ARG
      * for a level the last calc did not solve.  TV-L1: an OR of b2f_tvl1_path flags.  A shape whose tensor maps cannot
      * be encoded falls back to the plain-load kernels; this says whether it did.  Farneback: the b2f_farneback_path of
      * the fused iteration kernel (0 with numIters = 0).  kernel_path 3 falls back to the fast kernel on levels with
-     * fewer than 2 x n_SM 64x64 tiles or whose tensor maps cannot be encoded; this says whether it did. */
+     * fewer than 2 x n_SM 64x64 tiles or whose tensor maps cannot be encoded; this says whether it did.  Brox: the
+     * b2f_brox_path of the solver in bits 0-7, and in bits 8-15 the solver iterations the first launch of each inner
+     * step runs (all of them on a level that fits one 64x64 region or with B2F_BROX_PATH_COOP; the last launch of an
+     * inner step runs the remainder; 0 for B2F_BROX_PATH_HALF_SWEEP, whose launch is half an iteration; at most 255).
+     * kernel_path 3 falls back to kernel_path 0 on levels whose regions are not co-resident or that need more than one
+     * solver launch per inner step; this says whether it did. */
     B2F_ENGINE_ACTIVE_PATH = 1000
 } b2f_param_id;
 
@@ -203,6 +212,14 @@ typedef enum b2f_farneback_path {
     B2F_FARN_PATH_FAST = 7,            /* register-blocked, per-pixel R1 gather (kernel_path 2)                      */
     B2F_FARN_PATH_GENERIC = 8          /* k_farn_iter: any winSize other than 13, or kernel_path 1                   */
 } b2f_farneback_path;
+
+/* Brox solver kernels (B2F_ENGINE_ACTIVE_PATH, bits 0-7). */
+typedef enum b2f_brox_path {
+    B2F_BROX_PATH_REG = 1,        /* register-resident fused red-black SOR, one prepare + solver launches per inner step */
+    B2F_BROX_PATH_SMEM = 2,       /* shared-memory fused red-black SOR (kernel_path 2)                                  */
+    B2F_BROX_PATH_HALF_SWEEP = 3, /* one launch per red or black half sweep (kernel_path 1)                             */
+    B2F_BROX_PATH_COOP = 4        /* all inner steps of the level in one cooperative launch (kernel_path 3)             */
+} b2f_brox_path;
 
 typedef enum b2f_tvl1_path {
     B2F_TVL1_PATH_ITER_TMA = 1,       /* inner iterations: a persistent TMA-staged blocked kernel (kernel_path 0, 3-12) */

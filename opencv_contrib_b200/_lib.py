@@ -156,6 +156,8 @@ PARAM = {
 TVL1_PATH = dict(iter_tma=1, iter_blocked=2, iter_unfused=4, warp_tiled=8, warp_untiled=16)
 # b2f_farneback_path values (include/b200flow.h)
 FARN_PATH = dict(tma=1, quad=2, quad_wide=3, quad_r80=4, quad_r64=5, quad_transposed=6, fast=7, generic=8)
+# b2f_brox_path values (include/b200flow.h); B2F_ENGINE_ACTIVE_PATH carries one in bits 0-7, iterations per launch in 8-15
+BROX_PATH = dict(reg=1, smem=2, half_sweep=3, coop=4)
 
 _lib = None
 

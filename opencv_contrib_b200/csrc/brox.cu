@@ -52,18 +52,23 @@ __device__ __forceinline__ int mirror_load(int i, int n) {  // load_array_elemen
     return clampi(i, 0, n - 1);
 }
 
+// Rounding: the Brox kernels spell out every multiply-add rounding with __fmaf_rn / __fmul_rn / __fadd_rn, exactly
+// where nvcc -O3 fused or did not fuse the plain expressions (oracle/brox_model.py restates them one for one).  Plain
+// operators remain only where no contraction is possible (a sum of loads, a product that feeds no addition).
+
 // Normalised-coordinate, linear, mirror-addressed fetch (software replacement of the texture unit).
 __device__ __forceinline__ float tex_bilinear(const Plane &P, int h, int w, float xn, float yn) {
-    const float xb = xn * (float)w - 0.5f, yb = yn * (float)h - 0.5f;
+    const float xb = __fmaf_rn(xn, (float)w, -0.5f), yb = __fmaf_rn(yn, (float)h, -0.5f);
     const float fx0 = floorf(xb), fy0 = floorf(yb);
-    const float ax = xb - fx0, ay = yb - fy0;
+    const float ax = __fsub_rn(xb, fx0), ay = __fsub_rn(yb, fy0);
+    const float bx = __fsub_rn(1.f, ax), by = __fsub_rn(1.f, ay);
     // keep the integer conversion safe for wild flows; mirror addressing is periodic anyway
     const int x0 = (int)fminf(fmaxf(fx0, -1.0e6f), 1.0e6f), y0 = (int)fminf(fmaxf(fy0, -1.0e6f), 1.0e6f);
     const int xa = mirror_tex(x0, w), xc = mirror_tex(x0 + 1, w);
     const int ya = mirror_tex(y0, h), yc = mirror_tex(y0 + 1, h);
-    const float top = __ldg(&P.at(ya, xa)) * (1.f - ax) + __ldg(&P.at(ya, xc)) * ax;
-    const float bot = __ldg(&P.at(yc, xa)) * (1.f - ax) + __ldg(&P.at(yc, xc)) * ax;
-    return top * (1.f - ay) + bot * ay;
+    const float top = __fmaf_rn(bx, __ldg(&P.at(ya, xa)), __fmul_rn(ax, __ldg(&P.at(ya, xc))));
+    const float bot = __fmaf_rn(bx, __ldg(&P.at(yc, xa)), __fmul_rn(ax, __ldg(&P.at(yc, xc))));
+    return __fmaf_rn(by, top, __fmul_rn(ay, bot));
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -71,17 +76,18 @@ __device__ __forceinline__ float tex_bilinear(const Plane &P, int h, int w, floa
 // ---------------------------------------------------------------------------------------------
 __device__ __forceinline__ float ss_line(const float *row, int sw, float xmin, float xmax, int ixmin, int ixmax,
                                          float fxmin, float cxmax) {
-    float wsum = 1.0f - xmin + fxmin;
-    float sum = __ldg(row + ixmin) * (1.0f - xmin + fxmin);
+    const float w0 = __fadd_rn(__fsub_rn(1.0f, xmin), fxmin), w1 = __fsub_rn(cxmax, xmax);
+    float wsum = w0;
+    float sum = __fmul_rn(__ldg(row + ixmin), w0);
     int sp = ixmin + 1;
     for (int ix = ixmin + 1; ix < ixmax; ++ix) {
-        sum += __ldg(row + min(sp, sw - 1));
+        sum = __fadd_rn(sum, __ldg(row + min(sp, sw - 1)));
         sp++;
-        wsum += 1.0f;
+        wsum = __fadd_rn(wsum, 1.0f);
     }
-    sum += __ldg(row + min(sp, sw - 1)) * (cxmax - xmax);
-    wsum += cxmax - xmax;
-    return sum / wsum;
+    sum = __fmaf_rn(w1, __ldg(row + min(sp, sw - 1)), sum);
+    wsum = __fadd_rn(wsum, w1);
+    return __fdiv_rn(sum, wsum);
 }
 
 __global__ void __launch_bounds__(256) k_brox_supersample(Plane s0, Plane s1, int sh, int sw, Plane d0, Plane d1, int dh,
@@ -91,30 +97,33 @@ __global__ void __launch_bounds__(256) k_brox_supersample(Plane s0, Plane s1, in
     if (ix >= dw || iy >= dh) return;
     const Plane src = blockIdx.z ? s1 : s0;
     const float rw = (float)sw, rh = (float)sh;
-    const float x = scale * (float)ix, y = scale * (float)iy;
-    const float xBegin = fmaxf(x - scale, 0.0f), xEnd = fminf(x + scale, rw - 1.0f);
-    const float yBegin = fmaxf(y - scale, 0.0f), yEnd = fminf(y + scale, rh - 1.0f);
+    // x = scale * ix is never rounded on its own: both bounds fuse the product
+    const float fx = (float)ix, fy = (float)iy;
+    const float xBegin = fmaxf(__fmaf_rn(fx, scale, -scale), 0.0f), xEnd = fminf(__fmaf_rn(fx, scale, scale), __fsub_rn(rw, 1.0f));
+    const float yBegin = fmaxf(__fmaf_rn(fy, scale, -scale), 0.0f), yEnd = fminf(__fmaf_rn(fy, scale, scale), __fsub_rn(rh, 1.0f));
     const float fxb = floorf(xBegin), cxe = ceilf(xEnd);
     const int iXBegin = (int)fxb, iXEnd = (int)cxe;
     const float fyb = floorf(yBegin), cye = ceilf(yEnd);
     const int iYBegin = (int)fyb, iYEnd = (int)cye;
     int ry = iYBegin;
-    float wsum = 1.0f - yBegin + fyb;
-    float sum = ss_line(src.row(ry), sw, xBegin, xEnd, iXBegin, iXEnd, fxb, cxe) * (1.0f - yBegin + fyb);
+    const float w0 = __fadd_rn(__fsub_rn(1.0f, yBegin), fyb), w1 = __fsub_rn(cye, yEnd);
+    float wsum = w0;
+    float sum = __fmul_rn(ss_line(src.row(ry), sw, xBegin, xEnd, iXBegin, iXEnd, fxb, cxe), w0);
     ry++;
     for (int yy = iYBegin + 1; yy < iYEnd; ++yy) {
-        sum += ss_line(src.row(min(ry, sh - 1)), sw, xBegin, xEnd, iXBegin, iXEnd, fxb, cxe);
+        sum = __fadd_rn(sum, ss_line(src.row(min(ry, sh - 1)), sw, xBegin, xEnd, iXBegin, iXEnd, fxb, cxe));
         ry++;
-        wsum += 1.0f;
+        wsum = __fadd_rn(wsum, 1.0f);
     }
-    sum += ss_line(src.row(min(ry, sh - 1)), sw, xBegin, xEnd, iXBegin, iXEnd, fxb, cxe) * (cye - yEnd);
-    wsum += cye - yEnd;
-    (blockIdx.z ? d1 : d0).at(iy, ix) = sum / wsum;
+    sum = __fmaf_rn(w1, ss_line(src.row(min(ry, sh - 1)), sw, xBegin, xEnd, iXBegin, iXEnd, fxb, cxe), sum);
+    wsum = __fadd_rn(wsum, w1);
+    (blockIdx.z ? d1 : d0).at(iy, ix) = __fdiv_rn(sum, wsum);
 }
 
 // ---------------------------------------------------------------------------------------------
 // derivative bank: {1,-8,0,8,-1}/12 with the reference's mirror rule (NS:1449-1501; NB:843-868)
 // pass 1: Ix0, Iy0 (from I0), Ix, Iy (from I1);  pass 2: Ixx = dx(Ix), Iyy = dy(Iy), Ixy = dx(Iy)
+// The taps are left to nvcc: a product by +-1, +-8 or 0 is exact, so fusing it into the sum cannot change a bit.
 // ---------------------------------------------------------------------------------------------
 __device__ __forceinline__ float d5_row(const Plane &P, int y, int x, int w) {
     float sum = 0.0f;
@@ -172,6 +181,13 @@ constexpr int PT_W = PB_X + 2, PT_H = PB_Y + 2;
 struct PrepTile {
     float u[PT_H][PT_W], du[PT_H][PT_W], v[PT_H][PT_W], dv[PT_H][PT_W];
 };
+// 0.5 / sqrt(u_x^2 + v_x^2 + u_y^2 + v_y^2 + EPS2); the differences themselves are plain sums of loads
+__device__ __forceinline__ float brox_diffusivity(float u_x, float v_x, float u_y, float v_y) {
+    float s = __fmaf_rn(u_x, u_x, __fmul_rn(v_x, v_x));
+    s = __fmaf_rn(u_y, u_y, s);
+    s = __fmaf_rn(v_y, v_y, s);
+    return __fdiv_rn(0.5f, __fsqrt_rn(__fadd_rn(s, EPS2)));
+}
 // diffusivity between (i,j) and (i-1,j)  (NB:188-204); (ty, tx) = tile coordinates of (j, i)
 __device__ __forceinline__ float brox_sx(const PrepTile &T, int ty, int tx) {
     const float u_x = T.u[ty][tx] + T.du[ty][tx] - T.u[ty][tx - 1] - T.du[ty][tx - 1];
@@ -180,7 +196,7 @@ __device__ __forceinline__ float brox_sx(const PrepTile &T, int ty, int tx) {
                                T.u[ty - 1][tx] - T.du[ty - 1][tx] - T.u[ty - 1][tx - 1] - T.du[ty - 1][tx - 1]);
     const float v_y = 0.25f * (T.v[ty + 1][tx] + T.dv[ty + 1][tx] + T.v[ty + 1][tx - 1] + T.dv[ty + 1][tx - 1] -
                                T.v[ty - 1][tx] - T.dv[ty - 1][tx] - T.v[ty - 1][tx - 1] - T.dv[ty - 1][tx - 1]);
-    return 0.5f / sqrtf(u_x * u_x + v_x * v_x + u_y * u_y + v_y * v_y + EPS2);
+    return brox_diffusivity(u_x, v_x, u_y, v_y);
 }
 // diffusivity between (i,j) and (i,j-1)  (NB:216-227)
 __device__ __forceinline__ float brox_sy(const PrepTile &T, int ty, int tx) {
@@ -190,7 +206,7 @@ __device__ __forceinline__ float brox_sy(const PrepTile &T, int ty, int tx) {
                                T.u[ty][tx - 1] - T.u[ty - 1][tx - 1] - T.du[ty][tx - 1] - T.du[ty - 1][tx - 1]);
     const float v_x = 0.25f * (T.v[ty][tx + 1] + T.v[ty - 1][tx + 1] + T.dv[ty][tx + 1] + T.dv[ty - 1][tx + 1] -
                                T.v[ty][tx - 1] - T.v[ty - 1][tx - 1] - T.dv[ty][tx - 1] - T.dv[ty - 1][tx - 1]);
-    return 0.5f / sqrtf(u_x * u_x + v_x * v_x + u_y * u_y + v_y * v_y + EPS2);
+    return brox_diffusivity(u_x, v_x, u_y, v_y);
 }
 
 // The texture fetches of prepare_sor_stage_1 (NB:352-383): I1 and its derivatives sampled at the warped
@@ -233,7 +249,9 @@ struct PrepShared {
     float sx[PB_Y][PB_X + 1];   // sx at tile columns 0..32
     float sy[PB_Y + 1][PB_X];   // sy at tile rows 0..8
 };
-template <bool CG>
+// EXACT_RSQ (aux_path 1, a test knob): the data term's reciprocal square root correctly rounded (__frsqrt_rn) instead
+// of rsqrtf (MUFU.RSQ, up to 2 ulp, bits unspecified), so that a float model can follow the engine bit for bit.
+template <bool CG, bool EXACT_RSQ>
 __device__ __forceinline__ void brox_prepare_chunk(const BroxLevelPlanes &P, int h, int w, float alpha, float gamma, int gx0,
                                                    int gy0, int tid, PrepShared &S, bool active) {
     PrepTile &T = S.T;
@@ -272,30 +290,34 @@ __device__ __forceinline__ void brox_prepare_chunk(const BroxLevelPlanes &P, int
     const float du = T.du[ty + 1][tx + 1], dv = T.dv[ty + 1][tx + 1];
     const float Iz = P.wIz.at(jg, ig), Ix = P.wIx.at(jg, ig), Ixz = P.wIxz.at(jg, ig), Ixy = P.wIxy.at(jg, ig);
     const float Ixx = P.wIxx.at(jg, ig), Iy = P.wIy.at(jg, ig), Iyz = P.wIyz.at(jg, ig), Iyy = P.wIyy.at(jg, ig);
-    const float q0 = Iz + Ix * du + Iy * dv;
-    const float q1 = Ixz + Ixx * du + Ixy * dv;
-    const float q2 = Iyz + Ixy * du + Iyy * dv;
-    float data_term = 0.5f * rsqrtf(q0 * q0 + gamma * (q1 * q1 + q2 * q2) + EPS2);
-    data_term /= alpha;
+    const float q0 = __fmaf_rn(dv, Iy, __fmaf_rn(du, Ix, Iz));
+    const float q1 = __fmaf_rn(dv, Ixy, __fmaf_rn(du, Ixx, Ixz));
+    const float q2 = __fmaf_rn(dv, Iyy, __fmaf_rn(du, Ixy, Iyz));
+    const float r2 = __fadd_rn(__fmaf_rn(q0, q0, __fmul_rn(gamma, __fmaf_rn(q1, q1, __fmul_rn(q2, q2)))), EPS2);
+    float data_term = __fmul_rn(0.5f, EXACT_RSQ ? __frsqrt_rn(r2) : rsqrtf(r2));
+    data_term = __fdiv_rn(data_term, alpha);
 
     const float sx = S.sx[ty][tx], sxr = S.sx[ty][tx + 1];
     const float sy = S.sy[ty][tx], syu = S.sy[ty + 1][tx];
 
-    P.num_dudv.at(jg, ig) = data_term * (Ix * Iy + gamma * Ixy * (Ixx + Iyy));
-    P.num_u.at(jg, ig) = data_term * (Ix * Iz + gamma * (Ixx * Ixz + Ixy * Iyz));
-    P.num_v.at(jg, ig) = data_term * (Iy * Iz + gamma * (Iyy * Iyz + Ixy * Ixz));
-    const float den_u = data_term * (Ix * Ix + gamma * (Ixy * Ixy + Ixx * Ixx));
-    const float den_v = data_term * (Iy * Iy + gamma * (Ixy * Ixy + Iyy * Iyy));
+    // which product of a sum of two products is fused is nvcc's choice, pinned here term by term
+    P.num_dudv.at(jg, ig) = __fmul_rn(data_term, __fmaf_rn(Ix, Iy, __fmul_rn(__fmul_rn(gamma, Ixy), __fadd_rn(Ixx, Iyy))));
+    P.num_u.at(jg, ig) = __fmul_rn(data_term, __fmaf_rn(Ix, Iz, __fmul_rn(gamma, __fmaf_rn(Ixx, Ixz, __fmul_rn(Ixy, Iyz)))));
+    P.num_v.at(jg, ig) = __fmul_rn(data_term, __fmaf_rn(Iy, Iz, __fmul_rn(gamma, __fmaf_rn(Ixy, Ixz, __fmul_rn(Iyy, Iyz)))));
+    // data_term * den + dsum is one rounding
+    const float den_u = __fmaf_rn(Ix, Ix, __fmul_rn(gamma, __fmaf_rn(Ixy, Ixy, __fmul_rn(Ixx, Ixx))));
+    const float den_v = __fmaf_rn(Iy, Iy, __fmul_rn(gamma, __fmaf_rn(Ixy, Ixy, __fmul_rn(Iyy, Iyy))));
     P.sx.at(jg, ig) = sx;
     P.sy.at(jg, ig) = sy;
-    const float dsum = sx + sxr + sy + syu;
-    P.inv_u.at(jg, ig) = 1.0f / (den_u + dsum);
-    P.inv_v.at(jg, ig) = 1.0f / (den_v + dsum);
+    const float dsum = __fadd_rn(__fadd_rn(__fadd_rn(sx, sxr), sy), syu);
+    P.inv_u.at(jg, ig) = __frcp_rn(__fmaf_rn(data_term, den_u, dsum));
+    P.inv_v.at(jg, ig) = __frcp_rn(__fmaf_rn(data_term, den_v, dsum));
 }
 
+template <bool EXACT_RSQ>
 __global__ void __launch_bounds__(PB_X *PB_Y) k_brox_prepare(BroxLevelPlanes P, int h, int w, float alpha, float gamma) {
     __shared__ PrepShared S;
-    brox_prepare_chunk<false>(P, h, w, alpha, gamma, blockIdx.x * PB_X, blockIdx.y * PB_Y, threadIdx.y * PB_X + threadIdx.x, S,
+    brox_prepare_chunk<false, EXACT_RSQ>(P, h, w, alpha, gamma, blockIdx.x * PB_X, blockIdx.y * PB_Y, threadIdx.y * PB_X + threadIdx.x, S,
                               true);
 }
 
@@ -639,6 +661,7 @@ __device__ __forceinline__ void brox_grid_barrier(unsigned *counter, unsigned nb
     __syncthreads();
 }
 
+template <bool EXACT_RSQ>
 __global__ void __launch_bounds__(S_THREADS, 1)
     k_brox_level_coop(BroxLevelPlanes P, Plane dun, Plane dvn, int h, int w, float alpha, float gamma, float omega, int inner,
                       int iters, int halo, int tile, int tiles_x, unsigned *barrier) {
@@ -657,7 +680,7 @@ __global__ void __launch_bounds__(S_THREADS, 1)
             const int c = c0 + half;
             const bool active = c < nchunks;
             const int cy = active ? c / chunks_x : 0, cx = active ? c - cy * chunks_x : 0;
-            brox_prepare_chunk<true>(Q, h, w, alpha, gamma, cx * PB_X, cy * PB_Y, t256, PS[half], active);
+            brox_prepare_chunk<true, EXACT_RSQ>(Q, h, w, alpha, gamma, cx * PB_X, cy * PB_Y, t256, PS[half], active);
             __syncthreads();  // the tiles are reused by the next round
         }
         brox_grid_barrier(barrier, gridDim.x, epoch);
@@ -673,15 +696,15 @@ __global__ void __launch_bounds__(256) k_brox_add(Plane u, Plane v, Plane du, Pl
     const int x = blockIdx.x * blockDim.x + threadIdx.x;
     const int y = blockIdx.y * blockDim.y + threadIdx.y;
     if (x >= w || y >= h) return;
-    u.at(y, x) = u.at(y, x) + du.at(y, x);
-    v.at(y, x) = v.at(y, x) + dv.at(y, x);
+    u.at(y, x) = __fadd_rn(u.at(y, x), du.at(y, x));
+    v.at(y, x) = __fadd_rn(v.at(y, x), dv.at(y, x));
 }
 
 // bicubic prolongation (NS:2172-2231) fused with ScaleVector (NB:952-961); u and v per launch
 __device__ __forceinline__ float brox_bicubic_coeff(float x_) {
     const float x = fabsf(x_);
-    if (x <= 1.0f) return x * x * (1.5f * x - 2.5f) + 1.0f;
-    if (x < 2.0f) return x * (x * (-0.5f * x + 2.5f) - 4.0f) + 2.0f;
+    if (x <= 1.0f) return __fmaf_rn(__fmul_rn(x, x), __fmaf_rn(x, 1.5f, -2.5f), 1.0f);
+    if (x < 2.0f) return __fmaf_rn(x, __fmaf_rn(x, __fmaf_rn(x, -0.5f, 2.5f), -4.0f), 2.0f);
     return 0.0f;
 }
 
@@ -692,21 +715,22 @@ __global__ void __launch_bounds__(256) k_brox_prolong(Plane su, Plane sv, int sh
     if (ix >= dw || iy >= dh) return;
     const Plane src = blockIdx.z ? sv : su;
     const float rw = (float)sw, rh = (float)sh;
-    const float x = scale * (float)ix, y = scale * (float)iy;
-    const float xmin = fmaxf(ceilf(x - 2.0f), 0.0f), xmax = fminf(floorf(x + 2.0f), rw - 1.0f);
-    const float ymin = fmaxf(ceilf(y - 2.0f), 0.0f), ymax = fminf(floorf(y + 2.0f), rh - 1.0f);
+    // x = scale * ix is never rounded on its own: every use fuses the product (x - 2, x + 2, x - cx)
+    const float fx = (float)ix, fy = (float)iy;
+    const float xmin = fmaxf(ceilf(__fmaf_rn(fx, scale, -2.0f)), 0.0f), xmax = fminf(floorf(__fmaf_rn(fx, scale, 2.0f)), __fsub_rn(rw, 1.0f));
+    const float ymin = fmaxf(ceilf(__fmaf_rn(fy, scale, -2.0f)), 0.0f), ymax = fminf(floorf(__fmaf_rn(fy, scale, 2.0f)), __fsub_rn(rh, 1.0f));
     float sum = 0.0f, wsum = 0.0f;
-    for (float cy = ymin; cy <= ymax; cy += 1.0f) {
-        for (float cx = xmin; cx <= xmax; cx += 1.0f) {
-            float wx = brox_bicubic_coeff(x - cx);
-            const float wy = brox_bicubic_coeff(y - cy);
-            wx *= wy;
-            sum += wx * __ldg(&src.at((int)cy, (int)cx));
-            wsum += wx;
+    for (float cy = ymin; cy <= ymax; cy = __fadd_rn(cy, 1.0f)) {
+        for (float cx = xmin; cx <= xmax; cx = __fadd_rn(cx, 1.0f)) {
+            float wx = brox_bicubic_coeff(__fmaf_rn(fx, scale, -cx));
+            const float wy = brox_bicubic_coeff(__fmaf_rn(fy, scale, -cy));
+            wx = __fmul_rn(wx, wy);
+            sum = __fmaf_rn(wx, __ldg(&src.at((int)cy, (int)cx)), sum);
+            wsum = __fadd_rn(wsum, wx);
         }
     }
-    const float r = (!wsum) ? 0.f : sum / wsum;
-    (blockIdx.z ? dv : du).at(iy, ix) = r * mul;
+    const float r = (!wsum) ? 0.f : __fdiv_rn(sum, wsum);
+    (blockIdx.z ? dv : du).at(iy, ix) = __fmul_rn(r, mul);
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -749,8 +773,11 @@ private:
            S_INVU, S_INVV, S_NDUDV, S_WIZ, S_WIX, S_WIXZ, S_WIXY, S_WIXX, S_WIY, S_WIYZ, S_WIYY, S_COUNT };
     float *extra_[2] = {};  // num_u, num_v
     unsigned *coop_barrier_ = nullptr;  // arrival counter of the cooperative level kernel (zeroed before every launch)
-    int coop_max_blocks_ = -1;          // co-resident CTAs of k_brox_level_coop on this device (0: cooperative launch unsupported)
-    bool coop_ok(int blocks);
+    int coop_max_blocks_[2] = {-1, -1}; // co-resident CTAs of k_brox_level_coop<aux_path == 1> on this device (0: unsupported)
+    bool coop_ok(int blocks, bool exact_rsq);
+    // b2f_brox_path | iterations per solver launch << 8, per solved level: of the last calc (B2F_ENGINE_ACTIVE_PATH)
+    // and of the captured graph
+    std::vector<int> level_paths_, graph_level_paths_;
     int num_sms_ = 0;       // SM count of this handle's device (launch-cost model of the fused solver)
     int final_ui_ = 0;      // which (u, v) buffer pair holds the result (fixed by the level count)
 
@@ -822,21 +849,23 @@ cudaError_t BroxEngine::ensure_workspace(int rows, int cols) {
     return cudaSuccess;
 }
 
-bool BroxEngine::coop_ok(int blocks) {
-    if (coop_max_blocks_ < 0) {
-        coop_max_blocks_ = 0;
+bool BroxEngine::coop_ok(int blocks, bool exact_rsq) {
+    int &max_blocks = coop_max_blocks_[exact_rsq];
+    if (max_blocks < 0) {
+        max_blocks = 0;
         int dev = 0, coop = 0, sms = 0, per_sm = 0;
         const size_t smem = sizeof(float) * 10 * SR * SR;
+        auto kern = exact_rsq ? k_brox_level_coop<true> : k_brox_level_coop<false>;
         if (cudaGetDevice(&dev) == cudaSuccess &&
             cudaDeviceGetAttribute(&coop, cudaDevAttrCooperativeLaunch, dev) == cudaSuccess && coop &&
             cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev) == cudaSuccess &&
-            cudaFuncSetAttribute(k_brox_level_coop, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) == cudaSuccess &&
-            cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_brox_level_coop, S_THREADS, smem) == cudaSuccess)
-            coop_max_blocks_ = per_sm * sms;
+            cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) == cudaSuccess &&
+            cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kern, S_THREADS, smem) == cudaSuccess)
+            max_blocks = per_sm * sms;
         cudaGetLastError();
-        if (getenv("B2F_BROX_NO_COOP")) coop_max_blocks_ = 0;
+        if (getenv("B2F_BROX_NO_COOP")) max_blocks = 0;
     }
-    return blocks > 0 && blocks <= coop_max_blocks_;
+    return blocks > 0 && blocks <= max_blocks;
 }
 
 void BroxEngine::solve(Ctx &c) {
@@ -926,8 +955,21 @@ void BroxEngine::solve(Ctx &c) {
         const int it1 = single ? P.solver_iterations : std::min(P.solver_iterations, it_best);
         const int halo1 = single ? 0 : 2 * it1, tile1 = single ? SR : SR - 2 * halo1;
         const int tx1 = single ? 1 : div_up(w, tile1), ty1 = single ? 1 : div_up(h, tile1);
+        const bool exact_rsq = knobs.aux_path == 1;
         const bool use_coop = knobs.kernel_path == 3 && it1 == P.solver_iterations && P.solver_iterations > 0 &&
-                              P.inner_iterations > 0 && coop_ok(tx1 * ty1);
+                              P.inner_iterations > 0 && coop_ok(tx1 * ty1, exact_rsq);
+        {
+            int path = B2F_BROX_PATH_REG, per_launch = single ? P.solver_iterations : std::min(P.solver_iterations, it_best);
+            if (use_coop) {
+                path = B2F_BROX_PATH_COOP;
+            } else if (knobs.kernel_path == 1) {
+                path = B2F_BROX_PATH_HALF_SWEEP;
+                per_launch = 0;  // a launch is half an iteration
+            } else if (knobs.kernel_path == 2) {
+                path = B2F_BROX_PATH_SMEM;
+            }
+            level_paths_[l] = path | std::min(per_launch, 255) << 8;
+        }
         if (use_coop) {
             c.check(cudaMemsetAsync(coop_barrier_, 0, sizeof(unsigned), c.stream));
             if (c.ok()) {
@@ -938,7 +980,8 @@ void BroxEngine::solve(Ctx &c) {
                 unsigned *bar_ = coop_barrier_;
                 void *args[] = {&Q, &dun, &dvn, &h_, &w_, &alpha_f, &gamma_f, &omega_f, &inner_, &iters_, &halo_, &tile_,
                                 &tx_, &bar_};
-                c.check(cudaLaunchCooperativeKernel(reinterpret_cast<const void *>(k_brox_level_coop), dim3(tx1 * ty1),
+                auto kern = exact_rsq ? k_brox_level_coop<true> : k_brox_level_coop<false>;
+                c.check(cudaLaunchCooperativeKernel(reinterpret_cast<const void *>(kern), dim3(tx1 * ty1),
                                                     dim3(S_THREADS), args, sor_reg_smem, c.stream));
                 c.post(CLS_SOR);
                 c.stats->iterations_run += it1 * P.inner_iterations;
@@ -949,8 +992,12 @@ void BroxEngine::solve(Ctx &c) {
             }
         }
         for (int in = 0; in < P.inner_iterations && !use_coop; ++in) {
-            B2F_LAUNCH(c, CLS_PREP, 104.0 * npx, k_brox_prepare, grid, block, 0, T, h, w, static_cast<float>(P.alpha),
-                       static_cast<float>(P.gamma));
+            if (exact_rsq)
+                B2F_LAUNCH(c, CLS_PREP, 104.0 * npx, k_brox_prepare<true>, grid, block, 0, T, h, w, static_cast<float>(P.alpha),
+                           static_cast<float>(P.gamma));
+            else
+                B2F_LAUNCH(c, CLS_PREP, 104.0 * npx, k_brox_prepare<false>, grid, block, 0, T, h, w,
+                           static_cast<float>(P.alpha), static_cast<float>(P.gamma));
             if (knobs.kernel_path != 1) {
                 int left = P.solver_iterations;
                 Plane cdu = T.du, cdv = T.dv, ndu = dun, ndv = dvn;
@@ -1029,6 +1076,7 @@ int BroxEngine::calc(const b2f_image *I0, const b2f_image *I1, b2f_image *flow, 
     if (!c.ok()) return finish(c, s);
     stats.levels = static_cast<int>(L_.levels.size());
     stats.iterations_run = 0;
+    level_paths_.assign(L_.levels.size(), 0);
 
     const ImageView v0{I0->data, I0->step, rows, cols, I0->type};
     const ImageView v1{I1->data, I1->step, rows, cols, I1->type};
@@ -1064,6 +1112,7 @@ int BroxEngine::calc(const b2f_image *I0, const b2f_image *I1, b2f_image *flow, 
                 c.check(g.err);
                 if (c.ok()) {
                     key_.rows = rows; key_.cols = cols; key_.P = P; key_.knobs = knobs; key_.base = L_.levels[0].I0.p;
+                    graph_level_paths_ = level_paths_;
                 } else {
                     destroy_graph();
                 }
@@ -1077,6 +1126,7 @@ int BroxEngine::calc(const b2f_image *I0, const b2f_image *I1, b2f_image *flow, 
                 stats.class_bytes[i] += g_cls_bytes_[i];
             }
             stats.iterations_run = g_iters_;
+            level_paths_ = graph_level_paths_;
         }
     } else {
         solve(c);
@@ -1106,7 +1156,12 @@ int BroxEngine::get_param(int id, double *v) const {
         case B2F_BROX_INNER_ITERATIONS: *v = P.inner_iterations; break;
         case B2F_BROX_OUTER_ITERATIONS: *v = P.outer_iterations; break;
         case B2F_BROX_SOLVER_ITERATIONS: *v = P.solver_iterations; break;
-        default: return B2F_BAD_ARG;
+        default:
+            if (id >= B2F_ENGINE_ACTIVE_PATH && id - B2F_ENGINE_ACTIVE_PATH < (int)level_paths_.size()) {
+                *v = level_paths_[id - B2F_ENGINE_ACTIVE_PATH];
+                break;
+            }
+            return B2F_BAD_ARG;
     }
     return B2F_OK;
 }

@@ -239,6 +239,12 @@ _accessors(FarnebackOpticalFlow, "farneback", {
 class BroxOpticalFlow(DenseOpticalFlow):
     """cv::cuda::BroxOpticalFlow (cudaoptflow.hpp:155-186)."""
 
+    def getActivePath(self, level: int):
+        """The solver the last calc ran on pyramid level `level`: (a _lib.BROX_PATH value, solver iterations the first
+        launch of each inner step ran) (B2F_ENGINE_ACTIVE_PATH)."""
+        v = int(self._get(PARAM["engine"]["active_path"] + level))
+        return v & 0xFF, (v >> 8) & 0xFF
+
 
 _accessors(BroxOpticalFlow, "brox", {
     "alpha": ("FlowSmoothness", float), "gamma": ("GradientConstancyImportance", float),

@@ -6,11 +6,9 @@
                    unmodified into oracle/_ref/libtvl1_ref.so (oracle/Makefile, oracle/ref_shim/)
   refbuild_*.npz   the same build on a second input (digest of the flow, to pin the C port bit for bit) and with an
                    initial flow (stride-8 sample); inputs are regenerated from oracle/synth.py and checked by digest
-  brox_720p.npz    BASELINE-size output of the numpy restatement oracle/brox_model.py (no CPU implementation exists
-                   upstream: "parity unpinned"), stored as float32 on a stride-4 grid plus full-resolution means --
-                   2 minutes of numpy.  DensePyrLK needs no fixture: its C model runs at 1080p in seconds
-                   (tests/test_denselk_fullsize_gpu.py)
-python tests/golden/make_golden.py [farneback] [tvl1] [refbuild] [brox]   (no argument = farneback + tvl1)"""
+Brox and DensePyrLK need no fixture: their C models run at full size in the tests themselves
+(tests/test_brox_fullsize_gpu.py, tests/test_denselk_fullsize_gpu.py).
+python tests/golden/make_golden.py [farneback] [tvl1] [refbuild]   (no argument = farneback + tvl1)"""
 import hashlib
 import os
 import sys
@@ -81,21 +79,3 @@ if "refbuild" in WHAT:
                         flow_s8=flow[::8, ::8].copy(), mean_u=float(flow[..., 0].mean(dtype=np.float64)), **case,
                         **{"kw_" + k: v for k, v in kw.items()})
     print("refbuild", flow.shape, float(flow[..., 0].mean()))
-
-
-def _model_fixture(name, I0, I1, flow, kw, seed, kind, dtype):
-    out = {"flow_s4": flow[::4, ::4].astype(np.float32), "shape": np.array(flow.shape[:2]), "seed": seed, "kind": kind,
-           "dtype": dtype, "sha1_I0": hashlib.sha1(np.ascontiguousarray(I0).tobytes()).hexdigest(),
-           "sha1_I1": hashlib.sha1(np.ascontiguousarray(I1).tobytes()).hexdigest(),
-           "mean_u": float(flow[..., 0].mean(dtype=np.float64)), "mean_v": float(flow[..., 1].mean(dtype=np.float64)),
-           "mean_abs": float(np.abs(flow).mean(dtype=np.float64))}
-    out.update({"kw_" + k: v for k, v in kw.items()})
-    np.savez_compressed(os.path.join(HERE, name), **out)
-    print(name, flow.shape, out["mean_u"], out["mean_v"])
-
-
-if "brox" in WHAT:  # BASELINE configs[3]: 1280x720, create(0.197, 50, 0.8, 10, 77, 10) (cudaoptflow/test/test_optflow.cpp:75-76)
-    from oracle import brox_model  # noqa: E402
-    kw = dict(alpha=0.197, gamma=50.0, scale_factor=0.8, inner_iterations=10, outer_iterations=77, solver_iterations=10)
-    I0, I1, _ = synth.make_pair(720, 1280, seed=0, kind="smooth", dtype="f32")
-    _model_fixture("brox_720p.npz", I0, I1, brox_model.calc(I0, I1, brox_model.BroxParams(**kw)), kw, 0, "smooth", "f32")

@@ -93,6 +93,9 @@ def test_active_path_ids_match_header():
     farn = {m.group(1).lower(): int(m.group(2)) for m in re.finditer(r"B2F_FARN_PATH_(\w+)\s*=\s*(\d+)", src)}
     assert farn == _lib.FARN_PATH
     assert len(set(farn.values())) == len(farn) and 0 not in farn.values()  # 0 means "no iteration ran"
+    brox = {m.group(1).lower(): int(m.group(2)) for m in re.finditer(r"B2F_BROX_PATH_(\w+)\s*=\s*(\d+)", src)}
+    assert brox == _lib.BROX_PATH
+    assert len(set(brox.values())) == len(brox) and 0 not in brox.values() and max(brox.values()) < 256  # bits 0-7
     assert int(re.search(r"B2F_ENGINE_ACTIVE_PATH\s*=\s*(\d+)", src).group(1)) == _lib.PARAM["engine"]["active_path"]
 
 

@@ -9,16 +9,17 @@ test_optflow.cpp:130-161) and recovery of a known synthetic motion.
 import numpy as np
 import pytest
 
-from oracle import synth, metrics, brox_model as bm, denselk_model as lk, denselk_model_native as lkn
+from oracle import synth, brox_model as bm, brox_model_native as bmn, denselk_model as lk, denselk_model_native as lkn
 
 pytestmark = pytest.mark.gpu
 
 
-def _brox(dev, I0, I1, graph=1, **kw):
+def _brox(dev, I0, I1, graph=1, aux=0, **kw):
     import torch
     import opencv_contrib_b200 as ocb
     alg = ocb.BroxOpticalFlow_create(**kw)
     alg.setEngineOption("use_graph", graph)
+    alg.setEngineOption("aux_path", aux)
     f = alg.calc(torch.from_numpy(I0).to(dev), torch.from_numpy(I1).to(dev))
     torch.cuda.synchronize()
     return f.cpu().numpy(), alg
@@ -26,18 +27,25 @@ def _brox(dev, I0, I1, graph=1, **kw):
 
 @pytest.mark.parametrize("h,w,kind", [(96, 128, "const"), (121, 163, "smooth")])
 def test_brox_matches_model(cuda_device, h, w, kind):
+    """With the data term's rsqrt correctly rounded (aux_path 1) the engine equals the model bit for bit; the C model
+    equals the numpy statement.  The production rsqrtf (aux_path 0) is bounded by 4x the distance between the exact
+    model and the model with the rsqrt moved by up to 2 ulp (tests/test_brox_fullsize_gpu.py)."""
     I0, I1, gt = synth.make_pair(h, w, seed=3, kind=kind, dtype="f32")
     kw = dict(alpha=0.197, gamma=50.0, scale_factor=0.8, inner_iterations=5, outer_iterations=77, solver_iterations=5)
     ref = bm.calc(I0, I1, bm.BroxParams(**kw))
+    assert np.array_equal(bmn.calc(I0, I1, bm.BroxParams(**kw)).view(np.int32), ref.view(np.int32))
     for graph in (0, 1):
-        got, alg = _brox(cuda_device, I0, I1, graph=graph, **kw)
+        got, alg = _brox(cuda_device, I0, I1, graph=graph, aux=1, **kw)
         assert np.isfinite(got).all()
-        # SOR with omega = 1.99 sits at the edge of divergence and amplifies rounding (FMA contraction on the
-        # GPU vs separate mul/add in numpy): measured mean 1e-3 .. 1e-2 px, max < 0.1 px
-        st = metrics.epe_stats(got, ref)
-        assert st["mean"] <= 2e-2 and st["p95"] <= 5e-2 and st["max"] <= 0.25, (graph, st)
+        assert np.array_equal(got.view(np.int32), ref.view(np.int32)), (graph, int((got != ref).any(axis=-1).sum()))
     assert alg.getStats()["levels"] == len(bm.pyramid_sizes(h, w, 0.8, 77))
     assert alg.getDefaultName() == "DenseOpticalFlow.BroxOpticalFlow"
+    got, _ = _brox(cuda_device, I0, I1, graph=1, **kw)
+    pert = bmn.calc(I0, I1, bm.BroxParams(**kw), "perturbed")
+    err, yard = np.abs(got - ref), np.abs(pert - ref)
+    for q in (0.5, 0.99, 1.0):
+        assert np.quantile(err, q) <= max(4 * np.quantile(yard, q), 1e-6), (q, float(np.quantile(err, q)),
+                                                                              float(np.quantile(yard, q)))
 
 
 @pytest.mark.parametrize("h,w,solver", [(150, 203, 7), (61, 64, 10), (300, 417, 10)])
@@ -149,33 +157,3 @@ def test_denselk_fast_kernel_bit_identical_to_generic(cuda_device, win_h, levels
         alg.setEngineOption("kernel_path", path)
         outs.append(alg.calc(d0, d1, torch.zeros((131, 177, 2), device=cuda_device)).cpu().numpy())
     assert np.array_equal(outs[0], outs[1]), float(np.abs(outs[0] - outs[1]).max())
-
-
-def _model_golden(name):
-    """BASELINE-size fixture written by tests/golden/make_golden.py from the numpy restatement: the flow on a stride-4
-    grid plus full-resolution means; inputs are re-synthesised from the stored seed and checked by SHA-1."""
-    import hashlib
-    import os
-    z = np.load(os.path.join(os.path.dirname(__file__), "golden", name))
-    h, w = (int(v) for v in z["shape"])
-    I0, I1, _ = synth.make_pair(h, w, seed=int(z["seed"]), kind=str(z["kind"]), dtype=str(z["dtype"]))
-    if hashlib.sha1(np.ascontiguousarray(I0).tobytes()).hexdigest() != str(z["sha1_I0"]) or \
-            hashlib.sha1(np.ascontiguousarray(I1).tobytes()).hexdigest() != str(z["sha1_I1"]):
-        pytest.skip("synthetic inputs differ from the ones the fixture was made from (other cv2 / numpy build)")
-    kw = {k[3:]: z[k].item() for k in z.files if k.startswith("kw_")}
-    return z, I0, I1, kw
-
-
-def test_brox_720p_baseline_config_vs_model_golden(cuda_device):
-    """BASELINE configs[3]: 1280x720, create(0.197, 50, 0.8, 10, 77, 10) -- the only parameter set the reference runs
-    (test_optflow.cpp:75-76) -- against tests/golden/brox_720p.npz (oracle/brox_model.py at full size, 2 minutes of
-    numpy; parity unpinned upstream: the reference's own golden file lives in opencv_extra).  Tolerances as in
-    test_brox_matches_model (SOR at omega = 1.99 amplifies rounding): mean, p95, max."""
-    z, I0, I1, kw = _model_golden("brox_720p.npz")
-    got, alg = _brox(cuda_device, I0, I1, **kw)
-    assert np.isfinite(got).all() and alg.getStats()["levels"] == 19          # 1280x720 ... 24x13 (SURVEY.md §8)
-    st = metrics.epe_stats(got[::4, ::4], z["flow_s4"])
-    assert st["mean"] <= 2e-2 and st["p95"] <= 5e-2 and st["max"] <= 0.25, st
-    assert abs(float(got[..., 0].mean(dtype=np.float64)) - float(z["mean_u"])) <= 5e-3
-    assert abs(float(got[..., 1].mean(dtype=np.float64)) - float(z["mean_v"])) <= 5e-3
-

@@ -37,12 +37,6 @@ for name in sorted(os.listdir(gold)):
     st = metrics.epe_stats(got, z["flow"], border=16)
     ncc = metrics.ncc_dissimilarity(got[16:-16, 16:-16], z["flow"][16:-16, 16:-16])
     print("TV-L1 golden %s (%s): %s, NCC dissimilarity %.3g" % (name, ", ".join("%s=%s" % kv for kv in kw.items()), fmt(st), ncc), flush=True)
-z, I0, I1, kw = B._model_golden("brox_720p.npz")
-got, alg = B._brox(dev, I0, I1, **kw)
-st = metrics.epe_stats(got[::4, ::4], z["flow_s4"])
-print("Brox 720p (10, 77, 10) vs full-size numpy model (stride-4 grid): %s; mean u %.5f vs %.5f, mean v %.5f vs %.5f; levels %d"
-      % (fmt(st), got[..., 0].mean(dtype=np.float64), float(z["mean_u"]), got[..., 1].mean(dtype=np.float64), float(z["mean_v"]),
-         alg.getStats()["levels"]), flush=True)
 from oracle import denselk_model_native as lkn  # noqa: E402
 I0, I1, _ = synth.make_pair(1080, 1920, seed=0, kind="smooth")
 got, _ = B._lk(dev, I0, I1, winSize=(13, 13), maxLevel=3, iters=30)

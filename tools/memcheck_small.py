@@ -15,6 +15,7 @@ for name, alg, a, b in [
         ("brox", ocb.BroxOpticalFlow_create(0.197, 50.0, 0.8, 2, 10, 7), f0, f1),
         ("brox-pp", ocb.BroxOpticalFlow_create(0.197, 50.0, 0.8, 2, 10, 3), f0, f1),
         ("brox-coop", ocb.BroxOpticalFlow_create(0.197, 50.0, 0.8, 3, 10, 5), f0, f1),
+        ("brox-exact-rsqrt", ocb.BroxOpticalFlow_create(0.197, 50.0, 0.8, 2, 10, 4), f0, f1),
         ("tvl1-skewed", ocb.OpticalFlowDual_TVL1_create(nscales=2, warps=2, epsilon=0.0, iterations=8), d0, d1),
         ("denselk", ocb.DensePyrLKOpticalFlow_create(maxLevel=2, iters=4), d0, d1),
         ("denselk-generic", ocb.DensePyrLKOpticalFlow_create(winSize=(9, 7), maxLevel=1, iters=3), d0, d1),
@@ -24,6 +25,8 @@ for name, alg, a, b in [
         alg.setEngineOption("kernel_path", 2)
     if name == "brox-coop":
         alg.setEngineOption("kernel_path", 3)
+    if name == "brox-exact-rsqrt":
+        alg.setEngineOption("aux_path", 1)
     if name == "tvl1-skewed":
         alg.setEngineOption("kernel_path", 12)
     if len(sys.argv) > 1 and not any(name.startswith(a) for a in sys.argv[1:]):
@@ -61,6 +64,16 @@ for name, (h, w), kw, kp, aux in [
     torch.cuda.synchronize()
     print(name, "ok", float(ff.abs().mean()), "active path", [alg.getActivePath(k) for k in range(alg.getStats()["levels"])],
           flush=True)
+# Brox at the edge shapes of tests/test_brox_fullsize_gpu.py, every solver path, correctly rounded data-term rsqrt
+for (h, w), kp in [((1, 37), 0), ((37, 1), 0), ((2, 2), 0), ((15, 200), 1), ((65, 63), 2), ((141, 203), 3)]:
+    g = torch.rand((2, h, w), generator=torch.Generator().manual_seed(h * w)).to(dev)
+    alg = ocb.BroxOpticalFlow_create(0.197, 50.0, 0.8, 2, 10, 3)
+    alg.setEngineOption("kernel_path", kp)
+    alg.setEngineOption("aux_path", 1)
+    alg.setEngineOption("use_graph", 0)
+    fb = alg.calc(g[0].contiguous(), g[1].contiguous())
+    torch.cuda.synchronize()
+    print("brox", (h, w), "kernel_path", kp, "ok", float(fb.abs().mean()), flush=True)
 mid = ocb.interpolateFrames(f0, f1, fl[..., 0].contiguous(), fl[..., 1].contiguous(), -fl[..., 0].contiguous(),
                             -fl[..., 1].contiguous(), 0.3)
 mid2 = ocb.interpolateFrames(f0, f1, fl[..., 0].contiguous(), fl[..., 1].contiguous(), -fl[..., 0].contiguous(),
