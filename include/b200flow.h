@@ -162,12 +162,8 @@ typedef enum b2f_param_id {
     B2F_ENGINE_FUSED_ITERS = 900, /* TV-L1: inner iterations fused per HBM pass (0 = auto)     */
     B2F_ENGINE_USE_GRAPH = 901,   /* capture the fixed schedule in a CUDA graph (default 1)    */
     B2F_ENGINE_KERNEL_PATH = 902, /* TV-L1: 0 = auto (persistent TMA kernel, centre tiles stored by TMA), 1 = unfused
-                                     reference-shaped kernels, 2 = blocked kernel without TMA, 3 = TMA kernel without
-                                     elect.sync, 4 = TMA loads with the STG epilogue, 5 = paired-strip TMA kernel
-                                     (two pixels per thread row), 6 / 7 = 2x2 / 2x1-cluster kernels, 8 = two warp groups half an
-                                     iteration apart, 9 = warps synchronise with their neighbours through mbarriers
-                                     (11 = 9 with the TMA-store epilogue), 12 = row-skewed iterations behind
-                                     split-phase mbarriers.  All bit-identical; 0 is the default.
+                                     reference-shaped kernels, 2 = blocked kernel without TMA; any other value runs
+                                     0.  All bit-identical.
                                      Brox: 0 = register-resident solver, one prepare + one solver launch per inner
                                      step, 1 = one launch per half sweep, 2 = shared-memory solver, 3 = all inner steps
                                      of a level in one cooperative launch.  All bit-identical.
@@ -177,9 +173,8 @@ typedef enum b2f_param_id {
                                      kernel on levels with at least 2 x n_SM 64x64 tiles (0 elsewhere).  All agree to
                                      rounding; 3 is bit-identical to 0.  */
     B2F_ENGINE_AUX_PATH = 903,    /* variant of the secondary kernels.  TV-L1 warp: 0 = tiled kernel (I1 window of a
-                                     64x32 tile staged in shared memory by TMA), 1 = tap-by-tap kernel (accumulation
-                                     in the reference's order), 2 / 3 = separable kernel at 32 / 40 registers; 0, 2
-                                     and 3 are bit-identical.  Farneback: fused iteration kernel
+                                     64x32 tile staged in shared memory by TMA), 3 = separable kernel on every level;
+                                     any other value runs 0.  Bit-identical.  Farneback: fused iteration kernel
                                      at 0 = 128 registers (2 blocks / SM), 3 = 80, 4 = 64 registers, 5 = R1 gather
                                      with lanes on consecutive pixels, 6 = the simpler polynomial
                                      expansion and vertical-blur kernels.  All bit-identical.
@@ -222,11 +217,11 @@ typedef enum b2f_brox_path {
 } b2f_brox_path;
 
 typedef enum b2f_tvl1_path {
-    B2F_TVL1_PATH_ITER_TMA = 1,       /* inner iterations: a persistent TMA-staged blocked kernel (kernel_path 0, 3-12) */
+    B2F_TVL1_PATH_ITER_TMA = 1,       /* inner iterations: the persistent TMA-staged blocked kernel                      */
     B2F_TVL1_PATH_ITER_BLOCKED = 2,   /* inner iterations: the blocked kernel with plain loads                          */
     B2F_TVL1_PATH_ITER_UNFUSED = 4,   /* inner iterations: the unfused estimate_u / estimate_dual pair                  */
     B2F_TVL1_PATH_WARP_TILED = 8,     /* warp: the tiled kernel, I1 window staged by TMA                                */
-    B2F_TVL1_PATH_WARP_UNTILED = 16   /* warp: the separable or tap-by-tap kernel                                       */
+    B2F_TVL1_PATH_WARP_UNTILED = 16   /* warp: the separable kernel                                                     */
 } b2f_tvl1_path;
 
 /* cv::medianBlur for CV_32FC1, ksize 3 or 5, replicated border, not in place: the primitive behind

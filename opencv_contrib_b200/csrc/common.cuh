@@ -145,7 +145,7 @@ struct EngineKnobs {
     int fused_iters = 0;  // 0 = auto
     int use_graph = 1;
     int kernel_path = 0;  // 0 auto, 1 unfused reference-shaped kernels
-    int aux_path = 0;     // variant of the secondary kernels (TV-L1 warp: 0 tiled / TMA-staged, 1 tap-by-tap, 2 / 3 separable)
+    int aux_path = 0;     // variant of the secondary kernels (TV-L1 warp: 0 tiled / TMA-staged, 3 separable)
 };
 
 // Field-wise equality of the public parameter structs (they contain padding after int members, so memcmp on

@@ -44,87 +44,6 @@ struct Tvl1Planes {
 // for a zero gradient) instead of |grad|^2 itself: every consumer wants the reciprocal, it is constant over a warp's
 // inner iterations, and the iteration kernels used to recompute it for every tile of every pass.
 // ---------------------------------------------------------------------------------------------
-__global__ void __launch_bounds__(256) k_tvl1_warp(Plane I0, Plane I1, Plane u1p, Plane u2p, Plane I1wx, Plane I1wy,
-                                                   Plane grad, Plane rho, int rows, int cols) {
-    const int x = blockIdx.x * blockDim.x + threadIdx.x;
-    const int y = blockIdx.y * blockDim.y + threadIdx.y;
-    if (x >= cols || y >= rows) return;
-
-    // all three streaming operands first: the I0 load used to sit behind the first three stores (possible aliasing
-    // kept the compiler from hoisting it), a third dependent memory round trip per thread
-    const float u1 = __ldg(&u1p.at(y, x));
-    const float u2 = __ldg(&u2p.at(y, x));
-    const float I0v = __ldg(&I0.at(y, x));
-    const float wx = x + u1;
-    const float wy = y + u2;
-    const float fx = floorf(wx), fy = floorf(wy);
-    // integer tap origin, kept in a range where int conversion is safe even for wild flows
-    const int ix = static_cast<int>(fminf(fmaxf(fx, -8.f), cols + 8.f)) - 1;
-    const int iy = static_cast<int>(fminf(fmaxf(fy, -8.f), rows + 8.f)) - 1;
-
-    float kx[4], ky[4];
-#pragma unroll
-    for (int i = 0; i < 4; ++i) {
-        kx[i] = bicubic_coeff(wx - (fx + (i - 1)));
-        ky[i] = bicubic_coeff(wy - (fy + (i - 1)));
-    }
-
-    float sum = 0.f, sumx = 0.f, sumy = 0.f, wsum = 0.f;
-
-    if (ix >= 1 && iy >= 1 && ix + 4 <= cols - 1 && iy + 4 <= rows - 1) {
-        // interior: 6x6 window, no clamping
-        float win[6][6];
-        const float *base = &I1.at(iy - 1, ix - 1);
-#pragma unroll
-        for (int j = 0; j < 6; ++j)
-#pragma unroll
-            for (int i = 0; i < 6; ++i) win[j][i] = __ldg(base + (size_t)j * I1.pitch + i);
-#pragma unroll
-        for (int j = 0; j < 4; ++j) {
-#pragma unroll
-            for (int i = 0; i < 4; ++i) {
-                const float w = kx[i] * ky[j];
-                const float v = win[j + 1][i + 1];
-                const float gx = 0.5f * (win[j + 1][i + 2] - win[j + 1][i]);
-                const float gy = 0.5f * (win[j + 2][i + 1] - win[j][i + 1]);
-                sum = __fmaf_rn(w, v, sum);
-                sumx = __fmaf_rn(w, gx, sumx);
-                sumy = __fmaf_rn(w, gy, sumy);
-                wsum += w;
-            }
-        }
-    } else {
-        // border: clamp every tap, then take the clamped-neighbour gradient at the clamped tap
-#pragma unroll
-        for (int j = 0; j < 4; ++j) {
-            const int cy = clampi(iy + j, 0, rows - 1);
-            const int cyp = min(cy + 1, rows - 1), cym = max(cy - 1, 0);
-#pragma unroll
-            for (int i = 0; i < 4; ++i) {
-                const int cx = clampi(ix + i, 0, cols - 1);
-                const int cxp = min(cx + 1, cols - 1), cxm = max(cx - 1, 0);
-                const float w = kx[i] * ky[j];
-                const float v = __ldg(&I1.at(cy, cx));
-                const float gx = 0.5f * (__ldg(&I1.at(cy, cxp)) - __ldg(&I1.at(cy, cxm)));
-                const float gy = 0.5f * (__ldg(&I1.at(cyp, cx)) - __ldg(&I1.at(cym, cx)));
-                sum = __fmaf_rn(w, v, sum);
-                sumx = __fmaf_rn(w, gx, sumx);
-                sumy = __fmaf_rn(w, gy, sumy);
-                wsum += w;
-            }
-        }
-    }
-
-    const float coeff = 1.0f / wsum;
-    const float I1w = sum * coeff;
-    const float Ix = sumx * coeff;
-    const float Iy = sumy * coeff;
-    I1wx.at(y, x) = Ix;
-    I1wy.at(y, x) = Iy;
-    grad.at(y, x) = tvl1_inv_grad(__fmaf_rn(Iy, Iy, __fmul_rn(Ix, Ix)));  // the thresholding constant, not |grad|^2
-    rho.at(y, x) = __fsub_rn(__fmaf_rn(-Iy, u2, __fmaf_rn(-Ix, u1, I1w)), I0v);
-}
-
 // Border pixels of the warp (window touches the image edge): clamp every tap, then take the clamped-neighbour gradient
 // at the clamped tap (point / clamp texture semantics of tvl1flow.cu:106-164).  A real call on purpose.
 __device__ __noinline__ void warp_border_taps(const Plane I1, int rows, int cols, int ix, int iy, const float (&kx)[4],
@@ -149,8 +68,9 @@ __device__ __noinline__ void warp_border_taps(const Plane I1, int rows, int cols
     }
 }
 
-// Keys a = -0.5 weights of the four taps at distances (1 + t, t, 1 - t, 2 - t), t in [0, 1): the polynomials of
-// bicubic_coeff expanded in t (same values up to rounding; t itself is exact, the reference rounds t + 1 and 2 - t).
+// Keys a = -0.5 weights of the four taps at distances (1 + t, t, 1 - t, 2 - t), t in [0, 1): the reference's bicubic
+// polynomials (tvl1flow.cu:89-104) expanded in t (same values up to rounding; t itself is exact, the reference rounds
+// t + 1 and 2 - t).
 __device__ __forceinline__ void keys_weights(float t, float (&k)[4]) {
     k[0] = ((-0.5f * t + 1.0f) * t - 0.5f) * t;
     k[1] = (1.5f * t - 2.5f) * t * t + 1.0f;
@@ -158,11 +78,12 @@ __device__ __forceinline__ void keys_weights(float t, float (&k)[4]) {
     k[3] = (0.5f * t - 0.5f) * t * t;
 }
 
-// Separable form of the same warp (round 2; aux_path 3, and the fallback for levels smaller than one staged box): w_ij = kx[i] * ky[j], so the three weighted sums are row
-// sums r[j] = sum_i kx[i] W[j][i+1] (6 rows), rx[j] = sum_i kx[i] (W[j][i+2] - W[j][i]) (4 rows) combined with ky:
+// Separable form of the warp (round 2; aux_path 3, and the fallback for levels smaller than one staged box):
+// w_ij = kx[i] * ky[j], so the three weighted sums are row sums r[j] = sum_i kx[i] W[j][i+1] (6 rows),
+// rx[j] = sum_i kx[i] (W[j][i+2] - W[j][i]) (4 rows) combined with ky:
 //   I1w = sum_j ky[j] r[j+1],  I1wx = 0.5 sum_j ky[j] rx[j+1],  I1wy = 0.5 sum_j ky[j] (r[j+2] - r[j]),
-// about half the arithmetic of the tap-by-tap form (kept as aux_path 1; the few pixels whose window touches the image
-// border take its loop through an out-of-line call).  Results differ from the tap-by-tap accumulation by rounding only.
+// about half the arithmetic of the tap-by-tap form (the few pixels whose window touches the image border take the
+// tap-by-tap loop through an out-of-line call).  Results differ from the tap-by-tap accumulation by rounding only.
 // The warp kernel is bound by dependent memory round trips (flow -> window -> stores), not by arithmetic; what the
 // separable form buys is registers -- row by row it never holds the 6x6 window, fits 40 registers and runs 6 blocks
 // per SM instead of 4.
@@ -684,7 +605,7 @@ private:
     void proc_one_scale(Ctx &c, int s, Plane &u3cur, bool allow_sync);
     // epsilon > 0 inside a CUDA graph: the reference's adaptive loop as a WHILE conditional node (see EpsState)
     bool device_loop_ok() const {
-        return P.epsilon > 0.0 && !L_.gamma && tma_ok_ && (knobs.kernel_path == 0 || knobs.kernel_path == 3) &&
+        return P.epsilon > 0.0 && !L_.gamma && tma_ok_ && knobs.kernel_path == 0 &&
                median_filtering == 1 && !getenv("B2F_TVL1_HOST_LOOP");
     }
     void device_eps_loop(Ctx &c, int s, const Tvl1Planes &T, const Tvl1BlockedPlanes &B, const Tvl1Scalars &k,
@@ -855,8 +776,8 @@ void Tvl1Engine::device_eps_loop(Ctx &c, int s, const Tvl1Planes &T, const Tvl1B
         b.stream = bs;
         const double npx = (double)rows * cols;
         level_paths_[s] |= B2F_TVL1_PATH_ITER_TMA | B2F_TVL1_PATH_ITER_UNFUSED;
-        tvl1_tma_launch_dev(b, CLS_ITER, tma_maps(s, 0), B, 0, rows, cols, k, &L_.eps->ia, num_sms_, knobs.kernel_path == 0);
-        tvl1_tma_launch_dev(b, CLS_ITER, tma_maps(s, 1), B, 1, rows, cols, k, &L_.eps->ib, num_sms_, knobs.kernel_path == 0);
+        tvl1_tma_launch_dev(b, CLS_ITER, tma_maps(s, 0), B, 0, rows, cols, k, &L_.eps->ia, num_sms_);
+        tvl1_tma_launch_dev(b, CLS_ITER, tma_maps(s, 1), B, 1, rows, cols, k, &L_.eps->ib, num_sms_);
         B2F_LAUNCH(b, CLS_ITER, 48.0 * npx, k_tvl1_estimate_u, grid, block, 0, T, rows, cols, k, 1, L_.partials,
                    &L_.eps->sample);
         B2F_LAUNCH(b, CLS_REDUCE, 8.0 * nblocks, k_reduce_partials, dim3(1), dim3(256), 0, L_.partials, nblocks,
@@ -930,21 +851,8 @@ void Tvl1Engine::proc_one_scale(Ctx &c, int s, Plane &u3cur, bool allow_sync) {
         if (count > 0) level_paths_[s] |= use_tma ? B2F_TVL1_PATH_ITER_TMA : B2F_TVL1_PATH_ITER_BLOCKED;
         while (done < count) {
             const int kk = tvl1_blocked_pick_k(knobs.fused_iters, count - done, rows, cols);
-            if (use_tma && knobs.kernel_path == 5)  // paired-strip variant (two pixels per helper call)
-                tvl1_packed_launch(c, CLS_ITER, tma_maps(s, cur), B, cur, rows, cols, k, kk, num_sms_);
-            else if (use_tma && (knobs.kernel_path == 9 || knobs.kernel_path == 11))  // neighbour mbarriers (11: + TMA stores)
-                tvl1_tmanb_launch(c, CLS_ITER, tma_maps(s, cur), B, cur, rows, cols, k, kk, num_sms_, knobs.kernel_path == 11);
-            else if (use_tma && knobs.kernel_path == 12)  // row-skewed iterations behind split-phase barriers
-                tvl1_tmasp_launch(c, CLS_ITER, tma_maps(s, cur), B, cur, rows, cols, k, kk, num_sms_, true);
-            else if (use_tma && knobs.kernel_path == 8)  // two warp groups half an iteration apart
-                tvl1_tma2g_launch(c, CLS_ITER, tma_maps(s, cur), B, cur, rows, cols, k, kk, num_sms_);
-            else if (use_tma && (knobs.kernel_path == 6 || knobs.kernel_path == 7))  // 2x2 / 2x1 thread-block clusters
-                tvl1_cluster_launch(c, CLS_ITER, tma_maps(s, cur), B, cur, rows, cols, k, kk, num_sms_, 2,
-                                    knobs.kernel_path == 6 ? 2 : 1);
-            else if (use_tma)  // 0: the scalar persistent TMA kernel, centre tiles leave through TMA stores;
-                               // 4: the same with the STG epilogue; 3: 4 without elect.sync
-                tvl1_tma_launch(c, CLS_ITER, tma_maps(s, cur), B, cur, rows, cols, k, kk, num_sms_, knobs.kernel_path != 3,
-                                knobs.kernel_path != 3 && knobs.kernel_path != 4);
+            if (use_tma)  // the persistent TMA kernel
+                tvl1_tma_launch(c, CLS_ITER, tma_maps(s, cur), B, cur, rows, cols, k, kk, num_sms_);
             else
                 tvl1_blocked_launch(c, CLS_ITER, B, cur, rows, cols, k, kk);
             cur ^= 1;
@@ -970,25 +878,14 @@ void Tvl1Engine::proc_one_scale(Ctx &c, int s, Plane &u3cur, bool allow_sync) {
 
     for (int w = 0; w < P.warps; ++w) {
         point_T_at(cur);
-        // aux_path: 0 tiled (the default; levels smaller than one staged box take the separable kernel), 1 tap-by-tap in the
-        // reference's order (62 registers, 4 blocks / SM), 2 separable at 32 registers (8 blocks / SM), 3 separable at 40
-        // registers (6 blocks / SM; the default before the tiled kernel)
-        const bool tiled = (knobs.aux_path == 0 || knobs.aux_path == 4) && warp_maps_ && cols >= WB_W && rows >= WB_H;
+        // aux_path 3: the separable kernel on every level (40 registers, 6 blocks / SM; the default before the tiled
+        // kernel); any other value: the tiled kernel, levels smaller than one staged box the separable one
+        const bool tiled = knobs.aux_path != 3 && warp_maps_ && cols >= WB_W && rows >= WB_H;
         level_paths_[s] |= tiled ? B2F_TVL1_PATH_WARP_TILED : B2F_TVL1_PATH_WARP_UNTILED;
-        if (tiled && knobs.aux_path == 0)  // I1 window staged by the copy engine
+        if (tiled)  // I1 window staged by the copy engine
             B2F_LAUNCH(c, CLS_WARP, 32.0 * npx, k_tvl1_warp_tile<4>, dim3(div_up(cols, WT_W), div_up(rows, WT_H)),
                        dim3(WT_THREADS), 0, warp_maps_[s], lv.I0, lv.I1, T.u1, T.u2, T.I1wx, T.I1wy, T.grad, T.rho_c, rows,
                        cols);
-        else if (tiled)  // aux_path 4: the same at 77 registers, 3 blocks / SM
-            B2F_LAUNCH(c, CLS_WARP, 32.0 * npx, k_tvl1_warp_tile<3>, dim3(div_up(cols, WT_W), div_up(rows, WT_H)),
-                       dim3(WT_THREADS), 0, warp_maps_[s], lv.I0, lv.I1, T.u1, T.u2, T.I1wx, T.I1wy, T.grad, T.rho_c, rows,
-                       cols);
-        else if (knobs.aux_path == 1)
-            B2F_LAUNCH(c, CLS_WARP, 32.0 * npx, k_tvl1_warp, grid, block, 0, lv.I0, lv.I1, T.u1, T.u2, T.I1wx, T.I1wy,
-                       T.grad, T.rho_c, rows, cols);
-        else if (knobs.aux_path == 2)
-            B2F_LAUNCH(c, CLS_WARP, 32.0 * npx, k_tvl1_warp_sep<8>, grid, block, 0, lv.I0, lv.I1, T.u1, T.u2, T.I1wx,
-                       T.I1wy, T.grad, T.rho_c, rows, cols);
         else
             B2F_LAUNCH(c, CLS_WARP, 32.0 * npx, k_tvl1_warp_sep<6>, grid, block, 0, lv.I0, lv.I1, T.u1, T.u2, T.I1wx,
                        T.I1wy, T.grad, T.rho_c, rows, cols);

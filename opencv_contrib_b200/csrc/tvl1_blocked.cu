@@ -107,369 +107,6 @@ __device__ __forceinline__ void tile_iterate(Regs &r, float *ex, int iters, cons
     }
 }
 
-// ---------------------------------------------------------------------------------------------
-// Two-group variant of tile_iterate (kernel_path 8).  The two half iterations run in different regimes:
-// the primal update is FP32-issue bound, the dual update SFU / MIO-queue bound, and the CTA-wide barriers put all 16
-// warps into the same regime at the same time.  Here the upper half of the region (warps 0-7, group A) runs half an
-// iteration AHEAD of the lower half (warps 8-15, group B): while A's warps queue on the SFU in their dual update, B's
-// warps fill the FP32 issue slots with their primal update, and vice versa.
-//   * each group synchronises internally with its own named barrier (bar.sync 1 / 2, 256 threads);
-//   * B may start primal(it) only when A has finished primal(it) (A: bar.arrive 3, B: bar.sync 3) -- this is what keeps
-//     the groups half an iteration apart; A never waits for B in its primal update (up-neighbours only);
-//   * the seam rows cross between warp 7 and warp 8 only: warp 8 publishes its first row of u right after computing it
-//     and arrives on barrier 4, warp 7 syncs on it before it touches its last row in the dual update; warp 7 arrives on
-//     barrier 5 after publishing its last row of p, warp 8 syncs on it before its next primal update;
-//   * the exchange arrays are double-buffered by iteration parity, so a group that runs ahead never overwrites a row
-//     the other group still has to read.
-// Same arithmetic per pixel, same operands: bit-identical to tile_iterate.
-// ---------------------------------------------------------------------------------------------
-__device__ __forceinline__ void named_sync(int id, int count) { asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(count) : "memory"); }
-__device__ __forceinline__ void named_arrive(int id, int count) { asm volatile("bar.arrive %0, %1;" ::"r"(id), "r"(count) : "memory"); }
-
-template <bool BORDER>
-__device__ __forceinline__ void tile_iterate_2g(Regs &r, float *ex, int iters, const Tvl1Scalars k, int lx, int tr, int gxb,
-                                                int gyb, int W, int H) {
-    // ex: [parity][u1 | u2 | p12 | p22][32 thread rows][64]
-    const int mine = tr * R + 4 * lx;
-    const int up = max(tr - 1, 0) * R + 4 * lx;
-    const int dn = min(tr + 1, 31) * R + 4 * lx;
-    const int grp = tr >> 4;             // 0 = A (rows 0..31), 1 = B (rows 32..63)
-    const int warp = tr >> 1;            // 0..15
-    const int gbar = 1 + grp;
-
-
-    st4(ex + 2 * EX_F + mine, r.p12[1]);   // parity 0
-    st4(ex + 3 * EX_F + mine, r.p22[1]);
-    __syncthreads();
-
-    for (int it = 0; it < iters; ++it) {
-        float *exr = ex + (it & 1) * 4 * EX_F;        // u rows of this iteration / p rows read by this primal update
-        float *exw = ex + ((it + 1) & 1) * 4 * EX_F;  // p rows written by this dual update
-        if (grp == 1) named_sync(3, NT);              // B: not before A has finished primal(it)
-        // ---------------- primal update (estimateU) ----------------
-        if (warp == 8 && it > 0) named_sync(5, 64);   // A's last row of p (dual update it-1) is published
-        float up12[4], up22[4];
-        ld4(exr + 2 * EX_F + up, up12);
-        ld4(exr + 3 * EX_F + up, up22);
-#pragma unroll
-        for (int j = 0; j < 2; ++j) {
-            const float l11 = __shfl_up_sync(0xffffffffu, r.p11[j][3], 1, 16);
-            const float l21 = __shfl_up_sync(0xffffffffu, r.p21[j][3], 1, 16);
-#pragma unroll
-            for (int i = 0; i < 4; ++i) {
-                float pl11 = i ? r.p11[j][i ? i - 1 : 0] : l11;
-                float pl21 = i ? r.p21[j][i ? i - 1 : 0] : l21;
-                float pu12 = j ? r.p12[0][i] : up12[i];
-                float pu22 = j ? r.p22[0][i] : up22[i];
-                if (BORDER) {
-                    if (gxb + i == 0) { pl11 = 0.f; pl21 = 0.f; }
-                    if (gyb + j == 0) { pu12 = 0.f; pu22 = 0.f; }
-                }
-                float a, b;
-                tvl1_update_u(k, r.Ix[j][i], r.Iy[j][i], r.gr[j][i], r.rc[j][i], r.u1[j][i], r.u2[j][i], r.p11[j][i], pl11,
-                              r.p12[j][i], pu12, r.p21[j][i], pl21, r.p22[j][i], pu22, a, b);
-                r.u1[j][i] = a;
-                r.u2[j][i] = b;
-            }
-            if (j == 0) {  // the top row is what the thread row above needs: publish it as soon as it exists
-                st4(exr + mine, r.u1[0]);
-                st4(exr + EX_F + mine, r.u2[0]);
-                if (warp == 8) {
-                    __syncwarp();
-                    named_arrive(4, 64);  // B's first row of u is there for A's warp 7
-                }
-            }
-        }
-        if (grp == 0) named_arrive(3, NT);  // A has finished primal(it): B may start its own
-        named_sync(gbar, NT / 2);
-
-        // ---------------- dual update (estimateDualVariables) ----------------
-        float dn1[4], dn2[4];
-#pragma unroll
-        for (int j = 0; j < 2; ++j) {
-            if (j == 1) {  // the row below is only needed now; warp 7 takes it from group B, which runs half an iteration behind
-                if (warp == 7) named_sync(4, 64);
-                ld4(exr + dn, dn1);
-                ld4(exr + EX_F + dn, dn2);
-            }
-            const float r1 = __shfl_down_sync(0xffffffffu, r.u1[j][0], 1, 16);
-            const float r2 = __shfl_down_sync(0xffffffffu, r.u2[j][0], 1, 16);
-#pragma unroll
-            for (int i = 0; i < 4; ++i) {
-                const float c1 = r.u1[j][i], c2 = r.u2[j][i];
-                const float ur1 = i < 3 ? r.u1[j][i < 3 ? i + 1 : 3] : r1;
-                const float ur2 = i < 3 ? r.u2[j][i < 3 ? i + 1 : 3] : r2;
-                const float ud1 = j == 0 ? r.u1[1][i] : dn1[i];
-                const float ud2 = j == 0 ? r.u2[1][i] : dn2[i];
-                float ux1 = __fsub_rn(ur1, c1), uy1 = __fsub_rn(ud1, c1);
-                float ux2 = __fsub_rn(ur2, c2), uy2 = __fsub_rn(ud2, c2);
-                if (BORDER) {
-                    if (gxb + i == W - 1) { ux1 = 0.f; ux2 = 0.f; }
-                    if (gyb + j == H - 1) { uy1 = 0.f; uy2 = 0.f; }
-                }
-                tvl1_update_p2(k.taut, ux1, uy1, ux2, uy2, r.p11[j][i], r.p12[j][i], r.p21[j][i], r.p22[j][i]);
-            }
-        }
-        st4(exw + 2 * EX_F + mine, r.p12[1]);
-        st4(exw + 3 * EX_F + mine, r.p22[1]);
-        if (warp == 7 && it + 1 < iters) {
-            __syncwarp();
-            named_arrive(5, 64);  // A's last row of p is there for B's warp 8
-        }
-        named_sync(gbar, NT / 2);
-    }
-    __syncthreads();  // both groups are done with the tile (B half an iteration later)
-}
-
-
-// ---------------------------------------------------------------------------------------------
-// Neighbour-synchronised variant of tile_iterate (kernel_path 9).  In the default kernel the three CTA-wide
-// barriers of an iteration drain
-// all 16 warps at once (the dual update ends in a sqrt -> rcp -> mul chain), and they keep every warp of an SM
-// sub-partition in the same half iteration -- FP32-issue bound in the primal half, SFU-queue bound in the dual half.
-// But a warp (two thread rows = four pixel rows) only ever needs rows from the warp above (p12/p22, primal update)
-// and the warp below (u1/u2, dual update).  Here every warp owns two mbarriers (arrival count 1):
-//   done_p[w]: "warp w published the bottom rows of p"   -> waited on by warp w+1 before its primal update
-//   done_u[w]: "warp w published the top rows of u"      -> waited on by warp w-1 before its dual update
-// and no CTA-wide barrier is left inside the iterations.  Warps drift apart by up to one half iteration per warp of
-// distance, so the four warps of a sub-partition (w, w+4, w+8, w+12) sit in different halves and fill each other's
-// SFU / FP32 gaps.  mbarrier.try_wait suspends the warp in hardware; a waiting warp issues nothing.
-// Single-buffered exchange stays safe: warp w rewrites its u rows in primal(it) only after done_p[w-1] of dual(it-1),
-// by which time warp w-1 has read them; it rewrites its p rows in dual(it) only after done_u[w+1] of primal(it), by
-// which time warp w+1 has read them.  A producer is never more than one phase ahead of its consumer, so a parity bit
-// per waited barrier is enough.  Same arithmetic per pixel, same operands: bit-identical to tile_iterate.
-// ---------------------------------------------------------------------------------------------
-__device__ __forceinline__ uint32_t smem_u32_early(const void *p) { return (uint32_t)__cvta_generic_to_shared(p); }
-__device__ __forceinline__ void mbar_arrive_release(uint64_t *bar) {
-    asm volatile("mbarrier.arrive.release.cta.shared::cta.b64 _, [%0];" ::"r"(smem_u32_early(bar)) : "memory");
-}
-__device__ __forceinline__ void mbar_wait_parity(uint64_t *bar, uint32_t parity) {
-    asm volatile(
-        "{\n\t"
-        ".reg .pred p;\n\t"
-        "NB_WAIT:\n\t"
-        "mbarrier.try_wait.parity.acquire.cta.shared::cta.b64 p, [%0], %1;\n\t"
-        "@p bra NB_DONE;\n\t"
-        "bra NB_WAIT;\n\t"
-        "NB_DONE:\n\t"
-        "}" ::"r"(smem_u32_early(bar)), "r"(parity) : "memory");
-}
-
-template <bool BORDER>
-__device__ __forceinline__ void tile_iterate_nb(Regs &r, float *ex, uint64_t *nb, uint32_t &par_p, uint32_t &par_u,
-                                                int iters, const Tvl1Scalars k, int lx, int tr, int gxb, int gyb, int W,
-                                                int H) {
-    float *ex_u1 = ex, *ex_u2 = ex + EX_F, *ex_p12 = ex + 2 * EX_F, *ex_p22 = ex + 3 * EX_F;
-    const int mine = tr * R + 4 * lx;
-    const int up = max(tr - 1, 0) * R + 4 * lx;
-    const int dn = min(tr + 1, 31) * R + 4 * lx;
-    const int w = tr >> 1;
-    const bool lane0 = (threadIdx.x & 31) == 0;
-    uint64_t *done_p = nb, *done_u = nb + 16;
-
-    if (iters <= 0) return;
-
-    st4(ex_p12 + mine, r.p12[1]);
-    st4(ex_p22 + mine, r.p22[1]);
-    __syncwarp();
-    if (lane0) mbar_arrive_release(done_p + w);
-
-    for (int it = 0; it < iters; ++it) {
-        // ---------------- primal update ----------------
-        if (w > 0) {
-            mbar_wait_parity(done_p + (w - 1), par_p);
-            par_p ^= 1;
-        }
-        float up12[4], up22[4];
-        ld4(ex_p12 + up, up12);
-        ld4(ex_p22 + up, up22);
-#pragma unroll
-        for (int j = 0; j < 2; ++j) {
-            const float l11 = __shfl_up_sync(0xffffffffu, r.p11[j][3], 1, 16);
-            const float l21 = __shfl_up_sync(0xffffffffu, r.p21[j][3], 1, 16);
-#pragma unroll
-            for (int i = 0; i < 4; ++i) {
-                float pl11 = i ? r.p11[j][i ? i - 1 : 0] : l11;
-                float pl21 = i ? r.p21[j][i ? i - 1 : 0] : l21;
-                float pu12 = j ? r.p12[0][i] : up12[i];
-                float pu22 = j ? r.p22[0][i] : up22[i];
-                if (BORDER) {
-                    if (gxb + i == 0) { pl11 = 0.f; pl21 = 0.f; }
-                    if (gyb + j == 0) { pu12 = 0.f; pu22 = 0.f; }
-                }
-                float a, b;
-                tvl1_update_u(k, r.Ix[j][i], r.Iy[j][i], r.gr[j][i], r.rc[j][i], r.u1[j][i], r.u2[j][i],
-                              r.p11[j][i], pl11, r.p12[j][i], pu12, r.p21[j][i], pl21, r.p22[j][i], pu22, a, b);
-                r.u1[j][i] = a;
-                r.u2[j][i] = b;
-            }
-        }
-        st4(ex_u1 + mine, r.u1[0]);
-        st4(ex_u2 + mine, r.u2[0]);
-        __syncwarp();
-        if (lane0) mbar_arrive_release(done_u + w);
-
-        // ---------------- dual update ----------------
-        if (w < 15) {
-            mbar_wait_parity(done_u + (w + 1), par_u);
-            par_u ^= 1;
-        }
-        float dn1[4], dn2[4];
-        ld4(ex_u1 + dn, dn1);
-        ld4(ex_u2 + dn, dn2);
-#pragma unroll
-        for (int j = 0; j < 2; ++j) {
-            const float r1 = __shfl_down_sync(0xffffffffu, r.u1[j][0], 1, 16);
-            const float r2 = __shfl_down_sync(0xffffffffu, r.u2[j][0], 1, 16);
-#pragma unroll
-            for (int i = 0; i < 4; ++i) {
-                const float c1 = r.u1[j][i], c2 = r.u2[j][i];
-                const float ur1 = i < 3 ? r.u1[j][i < 3 ? i + 1 : 3] : r1;
-                const float ur2 = i < 3 ? r.u2[j][i < 3 ? i + 1 : 3] : r2;
-                const float ud1 = j == 0 ? r.u1[1][i] : dn1[i];
-                const float ud2 = j == 0 ? r.u2[1][i] : dn2[i];
-                float ux1 = __fsub_rn(ur1, c1), uy1 = __fsub_rn(ud1, c1);
-                float ux2 = __fsub_rn(ur2, c2), uy2 = __fsub_rn(ud2, c2);
-                if (BORDER) {
-                    if (gxb + i == W - 1) { ux1 = 0.f; ux2 = 0.f; }
-                    if (gyb + j == H - 1) { uy1 = 0.f; uy2 = 0.f; }
-                }
-                tvl1_update_p2(k.taut, ux1, uy1, ux2, uy2, r.p11[j][i], r.p12[j][i], r.p21[j][i], r.p22[j][i]);
-            }
-        }
-        if (it + 1 < iters) {  // the rows after the last dual update have no reader: keep arrivals and waits paired
-            st4(ex_p12 + mine, r.p12[1]);
-            st4(ex_p22 + mine, r.p22[1]);
-            __syncwarp();
-            if (lane0) mbar_arrive_release(done_p + w);
-        }
-    }
-}
-
-// ---------------------------------------------------------------------------------------------
-// Row-skewed variant of tile_iterate (kernel_path 12).  In the default kernel every warp runs into the
-// CTA barrier right after publishing its row, and the dual half iteration is bound by the SFU on its own.  But only ONE of a thread's two pixel rows depends on another thread in each half:
-//   P(top)    needs p(bottom row of the thread above)          P(bottom) needs this thread's own rows only
-//   D(bottom) needs u(top row of the thread below)             D(top)    needs this thread's own rows only
-// so the independent row is moved BEHIND the publication, between a split-phase arrive and its wait:
-//   wait B | P_n(top), publish u(top), arrive A | D_n(top) | wait A | D_n(bottom), publish p(bottom), arrive B | P_n+1(bottom)
-// Two mbarriers (one arrival per warp) replace the two __syncthreads; by the time a warp polls a barrier the other
-// warps had a four-pixel update's time to arrive, and SFU-heavy and FP32-only segments alternate twice per iteration.
-// Single-buffered exchange stays safe: u(top) is rewritten after wait B of the next iteration, i.e. after every warp
-// arrived on B, which each does after its read of the neighbour's u; p(bottom) is rewritten after wait A, which every
-// warp reaches after its read of the neighbour's p.  Same arithmetic per pixel, same operands: bit-identical.
-// ---------------------------------------------------------------------------------------------
-// split-phase barrier helpers on 32-bit shared addresses formed once per tile; the arrival is predicated, not branched
-__device__ __forceinline__ void sp_arrive(uint32_t bar_addr, uint32_t leader) {
-    asm volatile(
-        "{\n\t"
-        ".reg .pred p;\n\t"
-        "setp.ne.u32 p, %1, 0;\n\t"
-        "@p mbarrier.arrive.release.cta.shared::cta.b64 _, [%0];\n\t"
-        "}" ::"r"(bar_addr), "r"(leader) : "memory");
-}
-__device__ __forceinline__ void sp_wait(uint32_t bar_addr, uint32_t parity) {
-    asm volatile(
-        "{\n\t"
-        ".reg .pred p;\n\t"
-        "SP_WAIT:\n\t"
-        "mbarrier.try_wait.parity.acquire.cta.shared::cta.b64 p, [%0], %1;\n\t"
-        "@p bra SP_DONE;\n\t"
-        "bra SP_WAIT;\n\t"
-        "SP_DONE:\n\t"
-        "}" ::"r"(bar_addr), "r"(parity) : "memory");
-}
-
-template <bool BORDER, int J>
-__device__ __forceinline__ void sp_primal_row(Regs &r, const Tvl1Scalars &k, const float (&pu12)[4], const float (&pu22)[4],
-                                              int gxb, int gyb) {
-    const float l11 = __shfl_up_sync(0xffffffffu, r.p11[J][3], 1, 16);
-    const float l21 = __shfl_up_sync(0xffffffffu, r.p21[J][3], 1, 16);
-#pragma unroll
-    for (int i = 0; i < 4; ++i) {
-        float pl11 = i ? r.p11[J][i ? i - 1 : 0] : l11;
-        float pl21 = i ? r.p21[J][i ? i - 1 : 0] : l21;
-        float u12 = pu12[i], u22 = pu22[i];
-        if (BORDER) {
-            if (gxb + i == 0) { pl11 = 0.f; pl21 = 0.f; }
-            if (gyb + J == 0) { u12 = 0.f; u22 = 0.f; }
-        }
-        float a, b;
-        tvl1_update_u(k, r.Ix[J][i], r.Iy[J][i], r.gr[J][i], r.rc[J][i], r.u1[J][i], r.u2[J][i], r.p11[J][i], pl11,
-                      r.p12[J][i], u12, r.p21[J][i], pl21, r.p22[J][i], u22, a, b);
-        r.u1[J][i] = a;
-        r.u2[J][i] = b;
-    }
-}
-template <bool BORDER, int J>
-__device__ __forceinline__ void sp_dual_row(Regs &r, const Tvl1Scalars &k, const float (&dn1)[4], const float (&dn2)[4],
-                                            int gxb, int gyb, int W, int H) {
-    const float r1 = __shfl_down_sync(0xffffffffu, r.u1[J][0], 1, 16);
-    const float r2 = __shfl_down_sync(0xffffffffu, r.u2[J][0], 1, 16);
-#pragma unroll
-    for (int i = 0; i < 4; ++i) {
-        const float c1 = r.u1[J][i], c2 = r.u2[J][i];
-        const float ur1 = i < 3 ? r.u1[J][i < 3 ? i + 1 : 3] : r1;
-        const float ur2 = i < 3 ? r.u2[J][i < 3 ? i + 1 : 3] : r2;
-        float ux1 = __fsub_rn(ur1, c1), uy1 = __fsub_rn(dn1[i], c1);
-        float ux2 = __fsub_rn(ur2, c2), uy2 = __fsub_rn(dn2[i], c2);
-        if (BORDER) {
-            if (gxb + i == W - 1) { ux1 = 0.f; ux2 = 0.f; }
-            if (gyb + J == H - 1) { uy1 = 0.f; uy2 = 0.f; }
-        }
-        tvl1_update_p2(k.taut, ux1, uy1, ux2, uy2, r.p11[J][i], r.p12[J][i], r.p21[J][i], r.p22[J][i]);
-    }
-}
-
-template <bool BORDER>
-__device__ __forceinline__ void tile_iterate_sp(Regs &r, float *ex, uint64_t *ab, uint32_t &par_a, uint32_t &par_b, int iters,
-                                                const Tvl1Scalars k, int lx, int tr, int gxb, int gyb, int W, int H) {
-    float *ex_u1 = ex, *ex_u2 = ex + EX_F, *ex_p12 = ex + 2 * EX_F, *ex_p22 = ex + 3 * EX_F;
-    const int mine = tr * R + 4 * lx;
-    const int up = max(tr - 1, 0) * R + 4 * lx;
-    const int dn = min(tr + 1, 31) * R + 4 * lx;
-    const uint32_t lane0 = (threadIdx.x & 31) == 0 ? 1u : 0u;
-    // A: "u(top) published", B: "p(bottom) published"; 16 arrivals (one per warp) each
-    const uint32_t bar_a = smem_u32_early(ab), bar_b = bar_a + 8;
-
-    if (iters <= 0) return;
-
-    st4(ex_p12 + mine, r.p12[1]);
-    st4(ex_p22 + mine, r.p22[1]);
-    __syncwarp();
-    sp_arrive(bar_b, lane0);
-    sp_primal_row<BORDER, 1>(r, k, r.p12[0], r.p22[0], gxb, gyb);  // P_1(bottom): own rows only
-
-    for (int it = 0; it < iters; ++it) {
-        sp_wait(bar_b, par_b);
-        par_b ^= 1;
-        float up12[4], up22[4];
-        ld4(ex_p12 + up, up12);
-        ld4(ex_p22 + up, up22);
-        sp_primal_row<BORDER, 0>(r, k, up12, up22, gxb, gyb);
-        st4(ex_u1 + mine, r.u1[0]);
-        st4(ex_u2 + mine, r.u2[0]);
-        __syncwarp();
-        sp_arrive(bar_a, lane0);
-
-        sp_dual_row<BORDER, 0>(r, k, r.u1[1], r.u2[1], gxb, gyb, W, H);  // own rows only: runs while the others arrive
-
-        sp_wait(bar_a, par_a);
-        par_a ^= 1;
-        float dn1[4], dn2[4];
-        ld4(ex_u1 + dn, dn1);
-        ld4(ex_u2 + dn, dn2);
-        sp_dual_row<BORDER, 1>(r, k, dn1, dn2, gxb, gyb, W, H);
-        if (it + 1 < iters) {
-            st4(ex_p12 + mine, r.p12[1]);
-            st4(ex_p22 + mine, r.p22[1]);
-            __syncwarp();
-            sp_arrive(bar_b, lane0);
-            sp_primal_row<BORDER, 1>(r, k, r.p12[0], r.p22[0], gxb, gyb);  // P_n+1(bottom): own rows only
-        }
-    }
-}
-
 struct InPlanes {
     Plane p[N_IN];
 };
@@ -601,20 +238,6 @@ __device__ __forceinline__ void tma_store_2d(const CUtensorMap *map, const void 
                  ::"l"(reinterpret_cast<uint64_t>(map)), "r"(x), "r"(y), "r"(smem_u32(src)) : "memory");
 }
 
-// TMA needs the global address of every box row 16-byte aligned, i.e. the box x-origin a multiple
-// of 4 floats, while region origins are only even (tile*tx - halo).  The box is therefore 8 columns
-// wider than the region and starts at the region origin rounded down to a multiple of 4; threads
-// pick their pixels out of the staged rows at a 0- or 2-float shift (8-byte aligned LDS.64).
-// When the region origin is itself a multiple of 4 (halo and tile multiples of 4, e.g. K = 8) the box
-// is exactly the region (BOXW = 64) and threads read their pixels with conflict-free LDS.128.
-constexpr int TBOX_WIDE = R + 8;            // staged row length (floats), unaligned origins
-
-__device__ __forceinline__ void ld2x2(const float *s, float (&d)[4]) {
-    const float2 a = *reinterpret_cast<const float2 *>(s);
-    const float2 b = *reinterpret_cast<const float2 *>(s + 2);
-    d[0] = a.x; d[1] = a.y; d[2] = b.x; d[3] = b.y;
-}
-
 // One lane of a fully converged warp (the canonical TMA-issue guard: the branch is warp-uniform).
 __device__ __forceinline__ bool elect_one() {
     uint32_t pred = 0;
@@ -635,52 +258,43 @@ __device__ __forceinline__ void store_pairs(float *p, const float (&v)[4], int m
     else if (m1 == 1) p[2] = v[2];
 }
 
-// MODE 3 (measurement aid, tools/gpu_probe_tile_cost.py): the default kernel plus clock64 stamps of thread 0 around the
+// CLOCKS (measurement aid, tools/gpu_probe_tile_cost.py): the kernel plus clock64 stamps of thread 0 around the
 // phases of every tile, written to this buffer (8 values per tile: before wait, after wait, after fill, before the
 // iterations, after them, after the epilogue).
 __device__ long long *g_tvl1_clock_buf = nullptr;
 
-template <bool ELECT, int TBOX_W, int MODE = 0>  // MODE: 0 CTA barriers, 1 two groups, 2 neighbour mbarriers, 3 = 0 + clocks, 4 row-skewed
+// The halo is a multiple of 4 (tvl1_tma_launch), so every region origin is 16-byte aligned: the TMA box is exactly the
+// region and threads read their pixels out of the staged rows with conflict-free LDS.128.
+template <bool CLOCKS = false>
 __global__ void __launch_bounds__(NT, 1)
     k_tvl1_blocked_tma(const __grid_constant__ TmaMaps maps, Plane o_u1, Plane o_u2, Plane o_p11, Plane o_p12,
                        Plane o_p21, Plane o_p22, int rows, int cols, Tvl1Scalars k, int iters, int halo, int tile,
                        int tiles_x, int ntiles, const int *__restrict__ iters_dev,
                        const __grid_constant__ TmaOutMaps omaps, int tma_store) {
-    constexpr int TPLANE_F = TBOX_W * R;  // floats per staged plane
     if (iters_dev) {  // device-side convergence loop: the iteration count of this pass is decided on the GPU
         iters = __ldg(iters_dev);
         if (iters < 0) return;  // pass not needed (every thread takes the same branch)
     }
     extern __shared__ __align__(1024) float smem[];
     float *stage = smem;
-    float *ex = smem + N_IN * TPLANE_F;
-    constexpr bool TWOG = MODE == 1;
-    // two-group variant: exchange double-buffered; TMA-store epilogue: six output tiles alias the exchange arrays
-    constexpr int EX_AREA_F = TWOG ? 8 * EX_F : (TBOX_W == R ? (N_OUT * OT_F > 4 * EX_F ? N_OUT * OT_F : 4 * EX_F) : 4 * EX_F);
+    float *ex = smem + N_IN * PLANE_F;
+    // the six output tiles of the TMA-store epilogue alias the exchange arrays
+    constexpr int EX_AREA_F = N_OUT * OT_F > 4 * EX_F ? N_OUT * OT_F : 4 * EX_F;
     uint64_t *bar = reinterpret_cast<uint64_t *>(ex + EX_AREA_F);
-    uint64_t *nb = bar + 2;  // MODE 2: done_p[16], done_u[16]
-    uint32_t par_p = 0, par_u = 0;
 
     const int tid = threadIdx.x;
     const int lx = tid & 15, tr = tid >> 4;
-    constexpr uint32_t kStageBytes = N_IN * TPLANE_F * sizeof(float);
+    constexpr uint32_t kPlaneBytes = PLANE_F * sizeof(float);
 
-    // ELECT: the ten plane loads of a region are issued by ten warps (one elected lane each, each announcing its own
-    // 16 KB on the barrier), the six stores of the TMA-store epilogue by the other six.  One lane issuing all ten loads
-    // would put them on the critical path, every other warp waiting for it at the first barrier.
-    constexpr int LOAD_ISSUERS = ELECT ? N_IN : 1;
+    // The ten plane loads of a region are issued by ten warps (one elected lane each, each announcing its own 16 KB on
+    // the barrier), the six stores of the TMA-store epilogue by the other six.  One lane issuing all ten loads would
+    // put them on the critical path, every other warp waiting for it at the first barrier.
     const int wid = tid >> 5;
-    const bool leader = ELECT ? elect_one() : (tid == 0);         // one fixed lane per warp (ELECT) / thread 0
-    const bool load_issuer = ELECT ? (leader && wid < N_IN) : leader;
-    const bool store_issuer = ELECT ? (leader && wid >= N_IN && wid < N_IN + N_OUT) : leader;
+    const bool leader = elect_one();
+    const bool load_issuer = leader && wid < N_IN;
+    const bool store_issuer = leader && wid >= N_IN && wid < N_IN + N_OUT;
     if (tid == 0) {
-        mbar_init(bar, LOAD_ISSUERS);
-        if (MODE == 2)
-            for (int i = 0; i < 32; ++i) mbar_init(nb + i, 1);
-        if (MODE == 4) {
-            mbar_init(nb, NT / 32);
-            mbar_init(nb + 1, NT / 32);
-        }
+        mbar_init(bar, N_IN);
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
         asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
     }
@@ -693,15 +307,9 @@ __global__ void __launch_bounds__(NT, 1)
     tma_store &= 1;
     int t = blockIdx.x;
     auto issue_loads = [&](int tx, int ty) {
-        const int bx = (tx * tile - halo) & ~3, by = ty * tile - halo;
-        if (ELECT) {
-            mbar_expect_tx(bar, kStageBytes / N_IN);
-            tma_load_2d(stage + wid * TPLANE_F, &maps.in[wid], bx, by, bar);
-        } else {
-            mbar_expect_tx(bar, kStageBytes);
-#pragma unroll
-            for (int pl = 0; pl < N_IN; ++pl) tma_load_2d(stage + pl * TPLANE_F, &maps.in[pl], bx, by, bar);
-        }
+        const int bx = (tx * tile - halo) & ~3, by = ty * tile - halo;  // & ~3: see `shift` below
+        mbar_expect_tx(bar, kPlaneBytes);
+        tma_load_2d(stage + wid * PLANE_F, &maps.in[wid], bx, by, bar);
     };
     if (load_issuer && t < ntiles) {
         const int tt = rev ? ntiles - 1 - t : t;
@@ -713,24 +321,22 @@ __global__ void __launch_bounds__(NT, 1)
         const int tt = rev ? ntiles - 1 - t : t;
         const int ty = tt / tiles_x, tx = tt - ty * tiles_x;
         const int gx0 = tx * tile - halo, gy0 = ty * tile - halo;
-        const int shift = gx0 - (gx0 & ~3);  // 0 or 2
+        // Region origins are multiples of 4, so the rounding of the box origin above is a no-op and `shift` is 0.  Both
+        // stay: without them ptxas schedules the per-tile set-up differently, and a single-stream 1080p pair measured
+        // about 2 % slower on an H100.
+        const int shift = gx0 - (gx0 & ~3);
         long long clk[6];
-        if (MODE == 3) clk[0] = clock64();
+        if (CLOCKS) clk[0] = clock64();
         mbar_wait(bar, parity);
         parity ^= 1;
-        if (MODE == 3) clk[1] = clock64();
+        if (CLOCKS) clk[1] = clock64();
 
         Regs r;
         {
-            const int o0 = (2 * tr) * TBOX_W + shift + 4 * lx, o1 = o0 + TBOX_W;
+            const int o0 = (2 * tr) * R + shift + 4 * lx, o1 = o0 + R;
             auto ldrow = [&](int pl, float (&a)[4], float (&b)[4]) {
-                if (TBOX_W == R) {  // aligned origin: one 16-byte load per row
-                    ld4(stage + pl * TPLANE_F + o0, a);
-                    ld4(stage + pl * TPLANE_F + o1, b);
-                } else {
-                    ld2x2(stage + pl * TPLANE_F + o0, a);
-                    ld2x2(stage + pl * TPLANE_F + o1, b);
-                }
+                ld4(stage + pl * PLANE_F + o0, a);
+                ld4(stage + pl * PLANE_F + o1, b);
             };
             ldrow(0, r.Ix[0], r.Ix[1]);
             ldrow(1, r.Iy[0], r.Iy[1]);
@@ -743,10 +349,10 @@ __global__ void __launch_bounds__(NT, 1)
             ldrow(8, r.p21[0], r.p21[1]);
             ldrow(9, r.p22[0], r.p22[1]);
         }
-        if (TBOX_W == R && tma_store && store_issuer)  // the previous tile's TMA stores have read their staging tiles
+        if (tma_store && store_issuer)  // the previous tile's TMA stores have read their staging tiles
             asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory");
         __syncthreads();  // the staging buffer is free again
-        if (MODE == 3) clk[2] = clock64();
+        if (CLOCKS) clk[2] = clock64();
 
         // No proxy fence here: the generic-proxy reads of the staging buffer completed before the barrier above (their
         // values sit in registers); the copy engine only overwrites it (the consumer-release -> producer-load hand-off
@@ -760,34 +366,18 @@ __global__ void __launch_bounds__(NT, 1)
 
         const int gxb = gx0 + 4 * lx, gyb = gy0 + 2 * tr;
         const bool border = gx0 <= 0 || gy0 <= 0 || gx0 + R >= cols || gy0 + R >= rows;
-        if (MODE == 3) clk[3] = clock64();
-        if (MODE == 2) {
-            if (border)
-                tile_iterate_nb<true>(r, ex, nb, par_p, par_u, iters, k, lx, tr, gxb, gyb, cols, rows);
-            else
-                tile_iterate_nb<false>(r, ex, nb, par_p, par_u, iters, k, lx, tr, gxb, gyb, cols, rows);
-        } else if (MODE == 4) {
-            if (border)
-                tile_iterate_sp<true>(r, ex, nb, par_p, par_u, iters, k, lx, tr, gxb, gyb, cols, rows);
-            else
-                tile_iterate_sp<false>(r, ex, nb, par_p, par_u, iters, k, lx, tr, gxb, gyb, cols, rows);
-        } else if (TWOG) {
-            if (border)
-                tile_iterate_2g<true>(r, ex, iters, k, lx, tr, gxb, gyb, cols, rows);
-            else
-                tile_iterate_2g<false>(r, ex, iters, k, lx, tr, gxb, gyb, cols, rows);
-        } else if (border)
+        if (CLOCKS) clk[3] = clock64();
+        if (border)
             tile_iterate<true>(r, ex, iters, k, lx, tr, gxb, gyb, cols, rows);
         else
             tile_iterate<false>(r, ex, iters, k, lx, tr, gxb, gyb, cols, rows);
-        if (MODE == 3) clk[4] = clock64();
+        if (CLOCKS) clk[4] = clock64();
 
-        if (TBOX_W == R && tma_store) {
+        if (tma_store) {
             // centre tile -> six dense 48 x 48 tiles in shared memory (over the exchange arrays) -> one TMA store each.
             // 12 STS.128 per thread replace 24 predicated STG.64 and their address arithmetic; the copy engine clips
             // edge tiles against the image.  (halo == 8 and tile == 48 here.)
             float *ot = ex;
-            if (MODE == 2 || MODE == 4) __syncthreads();  // no CTA barrier ended the last dual update: neighbours may still read ex
             const int ox = 4 * lx - 8, oy = 2 * tr - 8;
             if (ox >= 0 && ox < OT) {
 #pragma unroll
@@ -806,15 +396,10 @@ __global__ void __launch_bounds__(NT, 1)
             asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
             __syncthreads();
             if (store_issuer) {
-                if (ELECT) {
-                    tma_store_2d(&omaps.out[wid - N_IN], ot + (wid - N_IN) * OT_F, tx * tile, ty * tile);
-                } else {
-#pragma unroll
-                    for (int pl = 0; pl < N_OUT; ++pl) tma_store_2d(&omaps.out[pl], ot + pl * OT_F, tx * tile, ty * tile);
-                }
+                tma_store_2d(&omaps.out[wid - N_IN], ot + (wid - N_IN) * OT_F, tx * tile, ty * tile);
                 asm volatile("cp.async.bulk.commit_group;" ::: "memory");
             }
-            if (MODE == 3 && tid == 0 && g_tvl1_clock_buf) {
+            if (CLOCKS && tid == 0 && g_tvl1_clock_buf) {
                 clk[5] = clock64();
 #pragma unroll
                 for (int i = 0; i < 6; ++i) g_tvl1_clock_buf[(size_t)t * 8 + i] = clk[i];
@@ -842,604 +427,8 @@ __global__ void __launch_bounds__(NT, 1)
             }
         }
     }
-    if (TBOX_W == R && tma_store && store_issuer)  // the staging tiles must outlive the copy engine's reads of them
+    if (tma_store && store_issuer)  // the staging tiles must outlive the copy engine's reads of them
         asm volatile("cp.async.bulk.wait_group 0;" ::: "memory");
-}
-
-
-// ---------------------------------------------------------------------------------------------
-// Paired-strip persistent TMA kernel (kernel_path 5).
-//
-// Same 64x64 region, same TMA staging, same arithmetic bit for bit -- but every thread now owns two
-// 4x1 pixel strips that are 32 rows apart: strip A in the upper half of the region (row tr) and strip B in
-// the lower half (row 32 + tr), and keeps each value as the pair (A, B).
-// Because the two strips are translates of one another, EVERY neighbour relation holds pairwise (the left
-// neighbour of (A, B) is (A_left, B_left), the upper one (A_up, B_up)), so the whole update runs on the
-// two-pixel helpers of tvl1_math.cuh with no repacking.
-// Vertical neighbours always belong to another thread row; they travel through four shared exchange arrays
-// whose slots hold ready-made (A, B) pairs:
-//   UP  (p12, p22): slot s = (row s-1, row 31+s), read by thread row s during the primal update
-//   DN  (u1,  u2 ): slot s = (row s+1, row 33+s), read by thread row s during the dual update
-// A thread row writes its natural pair to its neighbour's slot; only rows 31 / 32, where the halves meet,
-// are written as single elements (thread row 31 -> UP slot 0 .y, thread row 0 -> DN slot 31 .x).
-// Slot layout: [slot][half h = pixels 2h, 2h+1][lx] of float4 (A_2h, B_2h, A_2h+1, B_2h+1): consecutive lanes
-// read consecutive 16-byte words (conflict-free LDS.128 / STS.128).
-// Region origins are multiples of 4 (halo rounded up to a multiple of 4), so staging boxes are exactly the
-// region and the centre tile leaves as 16-byte vector stores.
-// ---------------------------------------------------------------------------------------------
-constexpr int PEX_F4 = 32 * 2 * 16;  // float4 per exchange array (32 slots x 2 halves x 16 lanes) = 16 KB
-
-struct RegsP {  // [i] = pixel column i of the thread's strips; .x = strip A (row tr), .y = strip B (row 32 + tr)
-    f2 Ix[4], Iy[4], ng[4], rc[4], u1[4], u2[4], p11[4], p12[4], p21[4], p22[4];
-};
-
-__device__ __forceinline__ void pex_publish(float4 *arr, int slot, int lx, const f2 (&v)[4]) {
-    arr[(slot * 2 + 0) * 16 + lx] = make_float4(v[0].x, v[0].y, v[1].x, v[1].y);
-    arr[(slot * 2 + 1) * 16 + lx] = make_float4(v[2].x, v[2].y, v[3].x, v[3].y);
-}
-__device__ __forceinline__ void pex_fetch(const float4 *arr, int slot, int lx, f2 (&v)[4]) {
-    const float4 a = arr[(slot * 2 + 0) * 16 + lx], b = arr[(slot * 2 + 1) * 16 + lx];
-    v[0] = make_float2(a.x, a.y); v[1] = make_float2(a.z, a.w);
-    v[2] = make_float2(b.x, b.y); v[3] = make_float2(b.z, b.w);
-}
-// thread row 31: its strip A (row 31) is the upper neighbour of thread row 0's strip B (row 32)
-__device__ __forceinline__ void pex_publish_up_seam(float4 *arr, int lx, const f2 (&v)[4]) {
-    float *f0 = reinterpret_cast<float *>(&arr[(0 * 2 + 0) * 16 + lx]);
-    float *f1 = reinterpret_cast<float *>(&arr[(0 * 2 + 1) * 16 + lx]);
-    f0[1] = v[0].x; f0[3] = v[1].x; f1[1] = v[2].x; f1[3] = v[3].x;
-}
-// thread row 0: its strip B (row 32) is the lower neighbour of thread row 31's strip A (row 31)
-__device__ __forceinline__ void pex_publish_dn_seam(float4 *arr, int lx, const f2 (&v)[4]) {
-    float *f0 = reinterpret_cast<float *>(&arr[(31 * 2 + 0) * 16 + lx]);
-    float *f1 = reinterpret_cast<float *>(&arr[(31 * 2 + 1) * 16 + lx]);
-    f0[0] = v[0].y; f0[2] = v[1].y; f1[0] = v[2].y; f1[2] = v[3].y;
-}
-__device__ __forceinline__ f2 shfl_up2(f2 v) {
-    return make_float2(__shfl_up_sync(0xffffffffu, v.x, 1, 16), __shfl_up_sync(0xffffffffu, v.y, 1, 16));
-}
-__device__ __forceinline__ f2 shfl_down2(f2 v) {
-    return make_float2(__shfl_down_sync(0xffffffffu, v.x, 1, 16), __shfl_down_sync(0xffffffffu, v.y, 1, 16));
-}
-
-// gx: global x of the thread's first pixel; gyA: global y of strip A (strip B is 32 rows below).
-template <bool BORDER>
-__device__ __forceinline__ void tile_iterate_packed(RegsP &r, float4 *ex, int iters, const Tvl1Scalars k, int lx,
-                                                    int tr, int gx, int gyA, int W, int H) {
-    float4 *up12 = ex, *up22 = ex + PEX_F4, *dn1 = ex + 2 * PEX_F4, *dn2 = ex + 3 * PEX_F4;
-    const int gyB = gyA + 32;
-
-#pragma unroll
-    for (int i = 0; i < 4; ++i) {  // thresholding constant, negated: rho * (-1/|grad|^2)
-        r.ng[i].x = -r.ng[i].x;
-        r.ng[i].y = -r.ng[i].y;
-    }
-
-    auto publish_up = [&]() {
-        if (tr < 31) { pex_publish(up12, tr + 1, lx, r.p12); pex_publish(up22, tr + 1, lx, r.p22); }
-        else { pex_publish_up_seam(up12, lx, r.p12); pex_publish_up_seam(up22, lx, r.p22); }
-    };
-    auto publish_dn = [&]() {
-        if (tr > 0) { pex_publish(dn1, tr - 1, lx, r.u1); pex_publish(dn2, tr - 1, lx, r.u2); }
-        else { pex_publish_dn_seam(dn1, lx, r.u1); pex_publish_dn_seam(dn2, lx, r.u2); }
-    };
-
-    publish_up();
-    __syncthreads();
-
-    for (int it = 0; it < iters; ++it) {
-        // ---------------- primal update (estimateU) ----------------
-        {
-            f2 u12[4], u22[4];
-            pex_fetch(up12, tr, lx, u12);
-            pex_fetch(up22, tr, lx, u22);
-            const f2 l11 = shfl_up2(r.p11[3]);
-            const f2 l21 = shfl_up2(r.p21[3]);
-#pragma unroll
-            for (int i = 0; i < 4; ++i) {
-                f2 pl11 = i ? r.p11[i ? i - 1 : 0] : l11;
-                f2 pl21 = i ? r.p21[i ? i - 1 : 0] : l21;
-                f2 pu12 = u12[i], pu22 = u22[i];
-                if (BORDER) {
-                    if (gx + i == 0) { pl11 = splat2(0.f); pl21 = splat2(0.f); }
-                    if (gyA == 0) { pu12.x = 0.f; pu22.x = 0.f; }
-                    if (gyB == 0) { pu12.y = 0.f; pu22.y = 0.f; }
-                }
-                f2 a, b;
-                tvl1_update_u_x2(k, r.Ix[i], r.Iy[i], r.ng[i], r.rc[i], r.u1[i], r.u2[i], r.p11[i], pl11, r.p12[i], pu12,
-                                 r.p21[i], pl21, r.p22[i], pu22, a, b);
-                r.u1[i] = a;
-                r.u2[i] = b;
-            }
-        }
-        publish_dn();
-        __syncthreads();
-
-        // ---------------- dual update (estimateDualVariables) ----------------
-        {
-            f2 d1[4], d2[4];
-            pex_fetch(dn1, tr, lx, d1);
-            pex_fetch(dn2, tr, lx, d2);
-            const f2 r1 = shfl_down2(r.u1[0]);
-            const f2 r2 = shfl_down2(r.u2[0]);
-#pragma unroll
-            for (int i = 0; i < 4; ++i) {
-                const f2 c1 = r.u1[i], c2 = r.u2[i];
-                const f2 ur1 = i < 3 ? r.u1[i < 3 ? i + 1 : 3] : r1;
-                const f2 ur2 = i < 3 ? r.u2[i < 3 ? i + 1 : 3] : r2;
-                f2 ux1 = sub2(ur1, c1), uy1 = sub2(d1[i], c1);
-                f2 ux2 = sub2(ur2, c2), uy2 = sub2(d2[i], c2);
-                if (BORDER) {
-                    if (gx + i == W - 1) { ux1 = splat2(0.f); ux2 = splat2(0.f); }
-                    if (gyA == H - 1) { uy1.x = 0.f; uy2.x = 0.f; }
-                    if (gyB == H - 1) { uy1.y = 0.f; uy2.y = 0.f; }
-                }
-                tvl1_update_p2_x2(k.taut, ux1, uy1, ux2, uy2, r.p11[i], r.p12[i], r.p21[i], r.p22[i]);
-            }
-        }
-        publish_up();
-        __syncthreads();
-    }
-}
-
-// one strip (4 pixels of one row) of one plane -> global; full = all four columns inside the image
-__device__ __forceinline__ void store_strip(float *p, float v0, float v1, float v2, float v3, bool full, int ncols) {
-    if (full) {
-        *reinterpret_cast<float4 *>(p) = make_float4(v0, v1, v2, v3);
-    } else {
-        if (ncols > 0) p[0] = v0;
-        if (ncols > 1) p[1] = v1;
-        if (ncols > 2) p[2] = v2;
-    }
-}
-
-__global__ void __launch_bounds__(NT, 1)
-    k_tvl1_packed_tma(const __grid_constant__ TmaMaps maps, Plane o_u1, Plane o_u2, Plane o_p11, Plane o_p12,
-                      Plane o_p21, Plane o_p22, int rows, int cols, Tvl1Scalars k, int iters, int halo, int tile,
-                      int tiles_x, int ntiles) {
-    extern __shared__ __align__(1024) float smem[];
-    float *stage = smem;
-    float4 *ex = reinterpret_cast<float4 *>(smem + N_IN * PLANE_F);
-    uint64_t *bar = reinterpret_cast<uint64_t *>(ex + 4 * PEX_F4);
-
-    const int tid = threadIdx.x;
-    const int lx = tid & 15, tr = tid >> 4;
-    constexpr uint32_t kStageBytes = N_IN * PLANE_F * sizeof(float);
-
-    if (tid == 0) {
-        mbar_init(bar, 1);
-        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-        asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-    }
-    // ghost halves of the seam slots (row -1 above the region, row 64 below it): never written afterwards
-    for (int i = tid; i < 4 * PEX_F4; i += NT) ex[i] = make_float4(0.f, 0.f, 0.f, 0.f);
-    __syncthreads();
-
-    int t = blockIdx.x;
-    const bool issuer = tid < 32 && elect_one();
-    if (issuer && t < ntiles) {
-        const int ty = t / tiles_x, tx = t - ty * tiles_x;
-        mbar_expect_tx(bar, kStageBytes);
-#pragma unroll
-        for (int pl = 0; pl < N_IN; ++pl)
-            tma_load_2d(stage + pl * PLANE_F, &maps.in[pl], tx * tile - halo, ty * tile - halo, bar);
-    }
-    uint32_t parity = 0;
-    for (; t < ntiles; t += gridDim.x) {
-        const int ty = t / tiles_x, tx = t - ty * tiles_x;
-        const int gx0 = tx * tile - halo, gy0 = ty * tile - halo;  // multiples of 4
-        mbar_wait(bar, parity);
-        parity ^= 1;
-
-        RegsP r;
-        {
-            const int oA = tr * R + 4 * lx, oB = oA + 32 * R;
-            auto ldpair = [&](int pl, f2 (&d)[4]) {
-                float a[4], b[4];
-                ld4(stage + pl * PLANE_F + oA, a);
-                ld4(stage + pl * PLANE_F + oB, b);
-                // x + (-0) == x bit for bit; the packed add makes ptxas materialise the (A, B) pair in an aligned
-                // register pair HERE, once per tile, instead of re-pairing the two LDS.128 results at every use
-#pragma unroll
-                for (int i = 0; i < 4; ++i) d[i] = add2(make_float2(a[i], b[i]), splat2(-0.0f));
-            };
-            ldpair(0, r.Ix);  ldpair(1, r.Iy);  ldpair(2, r.ng);  ldpair(3, r.rc);
-            ldpair(4, r.u1);  ldpair(5, r.u2);  ldpair(6, r.p11); ldpair(7, r.p12);
-            ldpair(8, r.p21); ldpair(9, r.p22);
-        }
-        __syncthreads();  // the staging buffer is free again
-
-        const int tn = t + gridDim.x;
-        if (issuer && tn < ntiles) {
-            const int ny = tn / tiles_x, nx = tn - ny * tiles_x;
-            asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-            mbar_expect_tx(bar, kStageBytes);
-#pragma unroll
-            for (int pl = 0; pl < N_IN; ++pl)
-                tma_load_2d(stage + pl * PLANE_F, &maps.in[pl], nx * tile - halo, ny * tile - halo, bar);
-        }
-
-        const int gxb = gx0 + 4 * lx, gyA = gy0 + tr;
-        const bool border = gx0 <= 0 || gy0 <= 0 || gx0 + R >= cols || gy0 + R >= rows;
-        if (border)
-            tile_iterate_packed<true>(r, ex, iters, k, lx, tr, gxb, gyA, cols, rows);
-        else
-            tile_iterate_packed<false>(r, ex, iters, k, lx, tr, gxb, gyA, cols, rows);
-
-        // centre tile -> global: 16-byte stores (gxb and the valid column range are multiples of 4)
-        const int rx = 4 * lx;
-        if (rx >= halo && rx < R - halo && gxb < cols) {
-            const bool full = gxb + 3 < cols;
-            const int nc = cols - gxb;
-#pragma unroll
-            for (int h = 0; h < 2; ++h) {
-                const int ry = tr + 32 * h, gy = gyA + 32 * h;
-                if (ry >= halo && ry < R - halo && gy < rows) {
-                    const size_t off = (size_t)gy * o_u1.pitch + gxb;
-                    auto st = [&](const Plane &P, const f2 (&v)[4]) {
-                        if (h == 0) store_strip(P.p + off, v[0].x, v[1].x, v[2].x, v[3].x, full, nc);
-                        else store_strip(P.p + off, v[0].y, v[1].y, v[2].y, v[3].y, full, nc);
-                    };
-                    st(o_u1, r.u1);   st(o_u2, r.u2);
-                    st(o_p11, r.p11); st(o_p12, r.p12);
-                    st(o_p21, r.p21); st(o_p22, r.p22);
-                }
-            }
-        }
-    }
-}
-
-
-// ---------------------------------------------------------------------------------------------
-// Thread-block-cluster variant (kernel_path 6 / 7): CX x CY CTAs of one cluster work on ONE super-region of
-// (64 CX) x (64 CY) pixels and exchange the one-pixel boundary of every half iteration through distributed shared
-// memory, so only the OUTER border of the super-region is halo: with K = 8 a 2 x 2 cluster keeps 112^2 of 128^2
-// computed pixels (76.6 %) where a lone CTA keeps 48^2 of 64^2 (56.3 %).
-//
-// Per CTA everything is as in k_tvl1_blocked_tma (64x64 region, 4x2 register micro-tiles, TMA-prefetched staging).
-// On top of it, per half iteration and per neighbouring CTA inside the cluster:
-//   after the dual update   my last column of (p11, p21) -> right neighbour's left ghost column,
-//                           my last row    of (p12, p22) -> lower neighbour's upper ghost row;
-//   after the primal update my first column of (u1, u2)  -> left neighbour's right ghost column,
-//                           my first row    of (u1, u2)  -> upper neighbour's lower ghost row.
-// Values travel as st.async (one 4-byte remote store each) that complete_tx on an mbarrier in the RECEIVING CTA; the
-// receiver arms that barrier with the byte count it expects and waits on it (acquire.cluster) at the start of the
-// half iteration that consumes the ghosts.  No cluster-wide barrier inside the loop: a CTA only ever waits for the
-// neighbours it reads from.  Such a hand-off costs a few hundred cycles one way; to keep it off the critical path every
-// half iteration computes the five pixels
-// of each micro-tile that need ghosts and produce the values to send FIRST, sends, and then computes the other three.
-// Overwrite safety needs no extra synchronisation: a neighbour can only produce the next value for a ghost cell after
-// it received what this CTA computed FROM the current one (the two hand-offs of an iteration depend on each other).
-// ---------------------------------------------------------------------------------------------
-struct ClusterGhosts {                 // 64 floats each, index = region row (columns) or region column (rows)
-    float p11L[R], p21L[R];            // left ghost column, read by the primal update of lx == 0
-    float p12U[R], p22U[R];            // upper ghost row,   read by the primal update of tr == 0
-    float u1R[R], u2R[R];              // right ghost column, read by the dual update of lx == 15
-    float u1D[R], u2D[R];              // lower ghost row,    read by the dual update of tr == 31
-};
-
-__device__ __forceinline__ uint32_t cluster_map(uint32_t smem_addr, uint32_t rank) {
-    uint32_t r;
-    asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(r) : "r"(smem_addr), "r"(rank));
-    return r;
-}
-__device__ __forceinline__ void st_async_f32(uint32_t remote_addr, float v, uint32_t remote_bar) {
-    asm volatile("st.async.weak.shared::cluster.mbarrier::complete_tx::bytes.b32 [%0], %1, [%2];" ::"r"(remote_addr),
-                 "r"(__float_as_uint(v)), "r"(remote_bar) : "memory");
-}
-// Waiting for ghosts = waiting on an mbarrier in MY shared memory whose tx-count the neighbours' st.async complete:
-// the default acquire at CTA scope orders my reads of the ghost cells behind it (the same wait TMA multicast uses).
-// An acquire.cluster here makes ptxas append CCTL.IVALL -- an L1 invalidate by all 512 threads twice per iteration.
-__device__ __forceinline__ void mbar_wait_cluster(uint64_t *bar, uint32_t parity) { mbar_wait(bar, parity); }
-__device__ __forceinline__ void cluster_sync_all() {
-    asm volatile("barrier.cluster.arrive.release.aligned;" ::: "memory");
-    asm volatile("barrier.cluster.wait.acquire.aligned;" ::: "memory");
-}
-
-// Per-thread role bits (one register instead of a dozen remote addresses: those are formed with one MAPA at send time).
-enum {
-    CR_LEFT = 1,     // lx == 0  and a left neighbour exists:  reads the left ghost column, sends its first column of u
-    CR_UP = 2,       // tr == 0  and an upper neighbour exists: reads the upper ghost row,  sends its first row of u
-    CR_RIGHT = 4,    // lx == 15 and a right neighbour exists: reads the right ghost column, sends its last column of p
-    CR_DOWN = 8,     // tr == 31 and a lower neighbour exists: reads the lower ghost row,   sends its last row of p
-    CR_WAIT_P = 16,  // this CTA receives ghosts for the primal update (it has a left or an upper neighbour)
-    CR_WAIT_U = 32,  // this CTA receives ghosts for the dual update (right or lower neighbour)
-    CR_ARM = 64      // thread 0: re-arms the ghost barriers
-};
-
-__device__ __forceinline__ void mbar_wait_addr(uint32_t bar_addr, uint32_t parity) {
-    asm volatile(
-        "{\n\t"
-        ".reg .pred p;\n\t"
-        "WAIT_LOOP_A:\n\t"
-        "mbarrier.try_wait.parity.shared::cta.b64 p, [%0], %1;\n\t"
-        "@p bra DONE_A;\n\t"
-        "bra WAIT_LOOP_A;\n\t"
-        "DONE_A:\n\t"
-        "}" ::"r"(bar_addr), "r"(parity) : "memory");
-}
-__device__ __forceinline__ void mbar_expect_tx_addr(uint32_t bar_addr, uint32_t bytes) {
-    asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(bar_addr), "r"(bytes) : "memory");
-}
-
-// K iterations with ghost exchange.  Same arithmetic, same operand order per pixel as tile_iterate.
-// gh_a / barP_a / barU_a: shared-window addresses of this CTA's ghost block and ghost barriers (the neighbours' copies
-// sit at the same offsets of THEIR windows: mapa).  nb_*: cluster ranks of the four neighbours.
-template <bool BORDER>
-__device__ __forceinline__ void tile_iterate_cluster(Regs &r, float *ex, const ClusterGhosts *gh, uint32_t gh_a,
-                                                     uint32_t barP_a, uint32_t barU_a, uint32_t role, uint32_t rank,
-                                                     uint32_t cluster_x, uint32_t bytes_p, uint32_t bytes_u,
-                                                     uint32_t &parP, uint32_t &parU, int iters, const Tvl1Scalars k, int lx,
-                                                     int tr, int gxb, int gyb, int W, int H) {
-    float *ex_u1 = ex, *ex_u2 = ex + EX_F, *ex_p12 = ex + 2 * EX_F, *ex_p22 = ex + 3 * EX_F;
-    const int mine = tr * R + 4 * lx;
-    const int up = max(tr - 1, 0) * R + 4 * lx;
-    const int dn = min(tr + 1, 31) * R + 4 * lx;
-    constexpr uint32_t OFF_P11L = offsetof(ClusterGhosts, p11L), OFF_P21L = offsetof(ClusterGhosts, p21L);
-    constexpr uint32_t OFF_P12U = offsetof(ClusterGhosts, p12U), OFF_P22U = offsetof(ClusterGhosts, p22U);
-    constexpr uint32_t OFF_U1R = offsetof(ClusterGhosts, u1R), OFF_U2R = offsetof(ClusterGhosts, u2R);
-    constexpr uint32_t OFF_U1D = offsetof(ClusterGhosts, u1D), OFF_U2D = offsetof(ClusterGhosts, u2D);
-
-
-    auto send_p = [&]() {  // my last column / last row of the dual variables -> right / lower neighbour
-        if (role & CR_RIGHT) {
-            const uint32_t g = cluster_map(gh_a, rank + 1), b = cluster_map(barP_a, rank + 1);
-#pragma unroll
-            for (int j = 0; j < 2; ++j) {
-                st_async_f32(g + OFF_P11L + 4u * (2 * tr + j), r.p11[j][3], b);
-                st_async_f32(g + OFF_P21L + 4u * (2 * tr + j), r.p21[j][3], b);
-            }
-        }
-        if (role & CR_DOWN) {
-            const uint32_t g = cluster_map(gh_a, rank + cluster_x), b = cluster_map(barP_a, rank + cluster_x);
-#pragma unroll
-            for (int i = 0; i < 4; ++i) {
-                st_async_f32(g + OFF_P12U + 4u * (4 * lx + i), r.p12[1][i], b);
-                st_async_f32(g + OFF_P22U + 4u * (4 * lx + i), r.p22[1][i], b);
-            }
-        }
-    };
-    auto send_u = [&]() {  // my first column / first row of the flow -> left / upper neighbour
-        if (role & CR_LEFT) {
-            const uint32_t g = cluster_map(gh_a, rank - 1), b = cluster_map(barU_a, rank - 1);
-#pragma unroll
-            for (int j = 0; j < 2; ++j) {
-                st_async_f32(g + OFF_U1R + 4u * (2 * tr + j), r.u1[j][0], b);
-                st_async_f32(g + OFF_U2R + 4u * (2 * tr + j), r.u2[j][0], b);
-            }
-        }
-        if (role & CR_UP) {
-            const uint32_t g = cluster_map(gh_a, rank - cluster_x), b = cluster_map(barU_a, rank - cluster_x);
-#pragma unroll
-            for (int i = 0; i < 4; ++i) {
-                st_async_f32(g + OFF_U1D + 4u * (4 * lx + i), r.u1[0][i], b);
-                st_async_f32(g + OFF_U2D + 4u * (4 * lx + i), r.u2[0][i], b);
-            }
-        }
-    };
-
-    st4(ex_p12 + mine, r.p12[1]);
-    st4(ex_p22 + mine, r.p22[1]);
-    send_p();
-    __syncthreads();
-
-    for (int it = 0; it < iters; ++it) {
-        // ---------------- primal update (estimateU) ----------------
-        {
-            float up12[4], up22[4], l11[2], l21[2];
-            ld4(ex_p12 + up, up12);
-            ld4(ex_p22 + up, up22);
-#pragma unroll
-            for (int j = 0; j < 2; ++j) {
-                l11[j] = __shfl_up_sync(0xffffffffu, r.p11[j][3], 1, 16);
-                l21[j] = __shfl_up_sync(0xffffffffu, r.p21[j][3], 1, 16);
-            }
-            if (role & CR_WAIT_P) {
-                mbar_wait_addr(barP_a, parP);
-                parP ^= 1;
-                if (role & CR_LEFT) {
-#pragma unroll
-                    for (int j = 0; j < 2; ++j) { l11[j] = gh->p11L[2 * tr + j]; l21[j] = gh->p21L[2 * tr + j]; }
-                }
-                if (role & CR_UP) {
-                    ld4(gh->p12U + 4 * lx, up12);
-                    ld4(gh->p22U + 4 * lx, up22);
-                }
-            }
-            auto px = [&](int j, int i) {
-                float pl11 = i ? r.p11[j][i ? i - 1 : 0] : l11[j];
-                float pl21 = i ? r.p21[j][i ? i - 1 : 0] : l21[j];
-                float pu12 = j ? r.p12[0][i] : up12[i];
-                float pu22 = j ? r.p22[0][i] : up22[i];
-                if (BORDER) {
-                    if (gxb + i == 0) { pl11 = 0.f; pl21 = 0.f; }
-                    if (gyb + j == 0) { pu12 = 0.f; pu22 = 0.f; }
-                }
-                float a, b;
-                tvl1_update_u(k, r.Ix[j][i], r.Iy[j][i], r.gr[j][i], r.rc[j][i], r.u1[j][i], r.u2[j][i], r.p11[j][i], pl11,
-                              r.p12[j][i], pu12, r.p21[j][i], pl21, r.p22[j][i], pu22, a, b);
-                r.u1[j][i] = a;
-                r.u2[j][i] = b;
-            };
-            // first the five pixels that read ghosts / feed the neighbours (row 0 and column 0), then the hand-off
-            px(0, 0); px(0, 1); px(0, 2); px(0, 3); px(1, 0);
-            send_u();
-            px(1, 1); px(1, 2); px(1, 3);
-        }
-        st4(ex_u1 + mine, r.u1[0]);
-        st4(ex_u2 + mine, r.u2[0]);
-        __syncthreads();
-        if ((role & (CR_WAIT_P | CR_ARM)) == (CR_WAIT_P | CR_ARM)) mbar_expect_tx_addr(barP_a, bytes_p);  // re-arm
-
-        // ---------------- dual update (estimateDualVariables) ----------------
-        {
-            float dn1[4], dn2[4], r1[2], r2[2];
-            ld4(ex_u1 + dn, dn1);
-            ld4(ex_u2 + dn, dn2);
-#pragma unroll
-            for (int j = 0; j < 2; ++j) {
-                r1[j] = __shfl_down_sync(0xffffffffu, r.u1[j][0], 1, 16);
-                r2[j] = __shfl_down_sync(0xffffffffu, r.u2[j][0], 1, 16);
-            }
-            if (role & CR_WAIT_U) {
-                mbar_wait_addr(barU_a, parU);
-                parU ^= 1;
-                if (role & CR_RIGHT) {
-#pragma unroll
-                    for (int j = 0; j < 2; ++j) { r1[j] = gh->u1R[2 * tr + j]; r2[j] = gh->u2R[2 * tr + j]; }
-                }
-                if (role & CR_DOWN) {
-                    ld4(gh->u1D + 4 * lx, dn1);
-                    ld4(gh->u2D + 4 * lx, dn2);
-                }
-            }
-            auto px = [&](int j, int i) {
-                const float c1 = r.u1[j][i], c2 = r.u2[j][i];
-                const float ur1 = i < 3 ? r.u1[j][i < 3 ? i + 1 : 3] : r1[j];
-                const float ur2 = i < 3 ? r.u2[j][i < 3 ? i + 1 : 3] : r2[j];
-                const float ud1 = j == 0 ? r.u1[1][i] : dn1[i];
-                const float ud2 = j == 0 ? r.u2[1][i] : dn2[i];
-                float ux1 = __fsub_rn(ur1, c1), uy1 = __fsub_rn(ud1, c1);
-                float ux2 = __fsub_rn(ur2, c2), uy2 = __fsub_rn(ud2, c2);
-                if (BORDER) {
-                    if (gxb + i == W - 1) { ux1 = 0.f; ux2 = 0.f; }
-                    if (gyb + j == H - 1) { uy1 = 0.f; uy2 = 0.f; }
-                }
-                tvl1_update_p2(k.taut, ux1, uy1, ux2, uy2, r.p11[j][i], r.p12[j][i], r.p21[j][i], r.p22[j][i]);
-            };
-            // first row 1 and column 3 (they read ghosts and produce what the neighbours wait for), then the hand-off
-            px(1, 0); px(1, 1); px(1, 2); px(1, 3); px(0, 3);
-            if (it + 1 < iters) send_p();   // the last dual update of a tile has no consumer: the next tile publishes afresh
-            px(0, 0); px(0, 1); px(0, 2);
-        }
-        st4(ex_p12 + mine, r.p12[1]);
-        st4(ex_p22 + mine, r.p22[1]);
-        __syncthreads();
-        if ((role & (CR_WAIT_U | CR_ARM)) == (CR_WAIT_U | CR_ARM)) mbar_expect_tx_addr(barU_a, bytes_u);
-    }
-}
-
-// cluster_x * cluster_y CTAs per cluster (rank = qy * cluster_x + qx); grid = clusters * cluster size, persistent over
-// super-tiles.  All CTAs of a cluster walk the same super-tile sequence (also the ones whose quadrant lies outside the
-// image: zero-filled by TMA, nothing stored), so the hand-off protocol is uniform.
-__global__ void __launch_bounds__(NT, 1)
-    k_tvl1_cluster_tma(const __grid_constant__ TmaMaps maps, Plane o_u1, Plane o_u2, Plane o_p11, Plane o_p12, Plane o_p21,
-                       Plane o_p22, int rows, int cols, Tvl1Scalars k, int iters, int halo, int cluster_x, int cluster_y,
-                       int stile_x, int stile_y, int stiles_x, int n_super) {
-    extern __shared__ __align__(1024) float smem[];
-    float *stage = smem;
-    float *ex = smem + N_IN * PLANE_F;
-    ClusterGhosts *gh = reinterpret_cast<ClusterGhosts *>(ex + 4 * EX_F);
-    uint64_t *bar = reinterpret_cast<uint64_t *>(gh + 1);  // [0] TMA staging, [1] ghosts of the primal update, [2] of the dual
-    uint64_t *barP = bar + 1, *barU = bar + 2;
-
-    const int tid = threadIdx.x;
-    const int lx = tid & 15, tr = tid >> 4;
-    constexpr uint32_t kStageBytes = N_IN * PLANE_F * sizeof(float);
-    const int csize = cluster_x * cluster_y;
-    uint32_t rank;
-    asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(rank));
-    const int qx = (int)rank % cluster_x, qy = (int)rank / cluster_x;
-    const int cluster_id = blockIdx.x / csize, n_clusters = gridDim.x / csize;
-
-    const bool has_left = qx > 0, has_right = qx < cluster_x - 1, has_up = qy > 0, has_down = qy < cluster_y - 1;
-    const uint32_t role = (has_left && lx == 0 ? CR_LEFT : 0u) | (has_up && tr == 0 ? CR_UP : 0u) |
-                          (has_right && lx == 15 ? CR_RIGHT : 0u) | (has_down && tr == 31 ? CR_DOWN : 0u) |
-                          (has_left || has_up ? CR_WAIT_P : 0u) | (has_right || has_down ? CR_WAIT_U : 0u) |
-                          (tid == 0 ? CR_ARM : 0u);
-    const uint32_t gh_a = smem_u32(gh), barP_a = smem_u32(barP), barU_a = smem_u32(barU);
-    const uint32_t bytes_p = (has_left ? 2u * R * 4u : 0u) + (has_up ? 2u * R * 4u : 0u);
-    const uint32_t bytes_u = (has_right ? 2u * R * 4u : 0u) + (has_down ? 2u * R * 4u : 0u);
-
-    if (tid == 0) {
-        mbar_init(bar, 1);
-        mbar_init(barP, 1);
-        mbar_init(barU, 1);
-        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-        asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-        if (bytes_p) mbar_expect_tx(barP, bytes_p);  // first phase of both ghost barriers
-        if (bytes_u) mbar_expect_tx(barU, bytes_u);
-    }
-    for (int i = tid; i < (int)(sizeof(ClusterGhosts) / sizeof(float)); i += NT) reinterpret_cast<float *>(gh)[i] = 0.f;
-    __syncthreads();
-    cluster_sync_all();  // nobody sends into a barrier that is not initialised yet
-
-    uint32_t parP = 0, parU = 0;
-    int st = cluster_id;
-    const bool issuer = tid < 32 && elect_one();
-    auto origin = [&](int s, int &ox, int &oy) {
-        const int sty = s / stiles_x, stx = s - sty * stiles_x;
-        ox = stx * stile_x - halo + R * qx;
-        oy = sty * stile_y - halo + R * qy;
-    };
-    if (issuer && st < n_super) {
-        int ox, oy;
-        origin(st, ox, oy);
-        mbar_expect_tx(bar, kStageBytes);
-#pragma unroll
-        for (int pl = 0; pl < N_IN; ++pl) tma_load_2d(stage + pl * PLANE_F, &maps.in[pl], ox, oy, bar);
-    }
-    uint32_t parity = 0;
-    for (; st < n_super; st += n_clusters) {
-        int gx0, gy0;
-        origin(st, gx0, gy0);
-        mbar_wait(bar, parity);
-        parity ^= 1;
-
-        Regs r;
-        {
-            const int o0 = (2 * tr) * R + 4 * lx, o1 = o0 + R;
-            auto ldrow = [&](int pl, float (&a)[4], float (&b)[4]) {
-                ld4(stage + pl * PLANE_F + o0, a);
-                ld4(stage + pl * PLANE_F + o1, b);
-            };
-            ldrow(0, r.Ix[0], r.Ix[1]);   ldrow(1, r.Iy[0], r.Iy[1]);   ldrow(2, r.gr[0], r.gr[1]);   ldrow(3, r.rc[0], r.rc[1]);
-            ldrow(4, r.u1[0], r.u1[1]);   ldrow(5, r.u2[0], r.u2[1]);   ldrow(6, r.p11[0], r.p11[1]); ldrow(7, r.p12[0], r.p12[1]);
-            ldrow(8, r.p21[0], r.p21[1]); ldrow(9, r.p22[0], r.p22[1]);
-        }
-        __syncthreads();  // the staging buffer is free again
-
-        const int sn = st + n_clusters;
-        if (issuer && sn < n_super) {
-            int ox, oy;
-            origin(sn, ox, oy);
-            asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-            mbar_expect_tx(bar, kStageBytes);
-#pragma unroll
-            for (int pl = 0; pl < N_IN; ++pl) tma_load_2d(stage + pl * PLANE_F, &maps.in[pl], ox, oy, bar);
-        }
-
-        const int gxb = gx0 + 4 * lx, gyb = gy0 + 2 * tr;
-        const bool border = gx0 <= 0 || gy0 <= 0 || gx0 + R >= cols || gy0 + R >= rows;
-        if (border)
-            tile_iterate_cluster<true>(r, ex, gh, gh_a, barP_a, barU_a, role, rank, (uint32_t)cluster_x, bytes_p, bytes_u,
-                                       parP, parU, iters, k, lx, tr, gxb, gyb, cols, rows);
-        else
-            tile_iterate_cluster<false>(r, ex, gh, gh_a, barP_a, barU_a, role, rank, (uint32_t)cluster_x, bytes_p, bytes_u,
-                                        parP, parU, iters, k, lx, tr, gxb, gyb, cols, rows);
-
-        // valid part of my region: the halo is only on the sides that are outer sides of the super-region
-        const int x_lo = has_left ? 0 : halo, x_hi = has_right ? R : R - halo;
-        const int y_lo = has_up ? 0 : halo, y_hi = has_down ? R : R - halo;
-        const int rx = 4 * lx;
-        if (rx >= x_lo && rx < x_hi && gxb >= 0 && gxb < cols) {
-            const bool full = gxb + 3 < cols;
-            const int nc = cols - gxb;
-#pragma unroll
-            for (int j = 0; j < 2; ++j) {
-                const int ry = 2 * tr + j, gy = gyb + j;
-                if (ry >= y_lo && ry < y_hi && gy >= 0 && gy < rows) {
-                    const size_t off = (size_t)gy * o_u1.pitch + gxb;
-                    store_strip(o_u1.p + off, r.u1[j][0], r.u1[j][1], r.u1[j][2], r.u1[j][3], full, nc);
-                    store_strip(o_u2.p + off, r.u2[j][0], r.u2[j][1], r.u2[j][2], r.u2[j][3], full, nc);
-                    store_strip(o_p11.p + off, r.p11[j][0], r.p11[j][1], r.p11[j][2], r.p11[j][3], full, nc);
-                    store_strip(o_p12.p + off, r.p12[j][0], r.p12[j][1], r.p12[j][2], r.p12[j][3], full, nc);
-                    store_strip(o_p21.p + off, r.p21[j][0], r.p21[j][1], r.p21[j][2], r.p21[j][3], full, nc);
-                    store_strip(o_p22.p + off, r.p22[j][0], r.p22[j][1], r.p22[j][2], r.p22[j][3], full, nc);
-                }
-            }
-        }
-    }
-    cluster_sync_all();  // no CTA leaves while a neighbour may still address its shared memory
 }
 
 }  // namespace
@@ -1465,12 +454,12 @@ static EncodeTiledFn get_encoder() {
     return fn;
 }
 
-static bool encode_plane(CUtensorMap *m, const Plane &P, int rows, int cols, int box_w) {
+static bool encode_plane(CUtensorMap *m, const Plane &P, int rows, int cols) {
     EncodeTiledFn enc = get_encoder();
     if (!enc) return false;
     const cuuint64_t gdim[2] = {(cuuint64_t)cols, (cuuint64_t)rows};
     const cuuint64_t gstr[1] = {(cuuint64_t)P.pitch * sizeof(float)};
-    const cuuint32_t box[2] = {(cuuint32_t)box_w, (cuuint32_t)R};
+    const cuuint32_t box[2] = {(cuuint32_t)R, (cuuint32_t)R};
     const cuuint32_t estr[2] = {1, 1};
     return enc(m, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, P.p, gdim, gstr, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
                CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
@@ -1492,19 +481,17 @@ bool tma_encode_2d_f32(void *map_out, const float *base, uint64_t width, uint64_
                CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
 }
 
-// one block = two input descriptor sets, [0] 72-wide boxes (any even origin), [1] 64-wide boxes (origin % 4 == 0),
-// followed by the output descriptors (48 x 48 boxes on the planes of the other state) of the TMA-store epilogue
-size_t tvl1_tma_maps_bytes() { return 2 * sizeof(TmaMaps) + sizeof(TmaOutMaps); }
+// one block = the input descriptors (64 x 64 boxes), followed by the output descriptors (48 x 48 boxes on the planes
+// of the other state) of the TMA-store epilogue
+size_t tvl1_tma_maps_bytes() { return sizeof(TmaMaps) + sizeof(TmaOutMaps); }
 
 bool tvl1_tma_build_maps(void *dst, const Tvl1BlockedPlanes &B, int cur, int rows, int cols) {
     TmaMaps *m = static_cast<TmaMaps *>(dst);
     const Tvl1State &si = B.s[cur];
     const Plane in[N_IN] = {B.I1wx, B.I1wy, B.grad, B.rho_c, si.u1, si.u2, si.p11, si.p12, si.p21, si.p22};
-    for (int i = 0; i < N_IN; ++i) {
-        if (!encode_plane(&m[0].in[i], in[i], rows, cols, TBOX_WIDE)) return false;
-        if (!encode_plane(&m[1].in[i], in[i], rows, cols, R)) return false;
-    }
-    TmaOutMaps *om = reinterpret_cast<TmaOutMaps *>(m + 2);
+    for (int i = 0; i < N_IN; ++i)
+        if (!encode_plane(&m->in[i], in[i], rows, cols)) return false;
+    TmaOutMaps *om = reinterpret_cast<TmaOutMaps *>(m + 1);
     const Tvl1State &so = B.s[cur ^ 1];
     const Plane out[N_OUT] = {so.u1, so.u2, so.p11, so.p12, so.p21, so.p22};
     for (int i = 0; i < N_OUT; ++i)
@@ -1514,46 +501,39 @@ bool tvl1_tma_build_maps(void *dst, const Tvl1BlockedPlanes &B, int cur, int row
     return true;
 }
 static const TmaOutMaps *out_maps(const void *maps) {
-    return reinterpret_cast<const TmaOutMaps *>(static_cast<const TmaMaps *>(maps) + 2);
+    return reinterpret_cast<const TmaOutMaps *>(static_cast<const TmaMaps *>(maps) + 1);
 }
 
-// exchange area: four exchange arrays; the 64-wide-box kernels keep room for the six 48 x 48 output tiles of the
-// TMA-store epilogue there (they alias the exchange arrays), the two-group kernel for its second set of arrays
-constexpr size_t ex_area_floats(int box_w, int mode) {
-    return mode == 1 ? 8 * (size_t)EX_F
-                     : (box_w == R && (size_t)N_OUT * OT_F > 4 * (size_t)EX_F ? (size_t)N_OUT * OT_F : 4 * (size_t)EX_F);
+// staged planes, then the four exchange arrays with room for the six 48 x 48 output tiles of the TMA-store epilogue
+// (they alias the exchange arrays), then the barrier
+constexpr size_t smem_tma_bytes() {
+    return sizeof(float) * ((size_t)N_IN * PLANE_F + ((size_t)N_OUT * OT_F > 4 * (size_t)EX_F ? (size_t)N_OUT * OT_F : 4 * (size_t)EX_F)) + 64;
 }
-constexpr size_t smem_tma_bytes(int box_w, int mode = 0) {
-    return sizeof(float) * ((size_t)N_IN * box_w * R + ex_area_floats(box_w, mode)) + 64 + (mode == 2 || mode == 4 ? 256 : 0);
-}
-static_assert(smem_tma_bytes(R, 0) <= 227 * 1024 && smem_tma_bytes(R, 1) <= 227 * 1024 && smem_tma_bytes(R, 2) <= 227 * 1024,
-              "TV-L1 TMA kernel: shared memory over the 227 KB limit");
+static_assert(smem_tma_bytes() <= 227 * 1024, "TV-L1 TMA kernel: shared memory over the 227 KB limit");
 
 void tvl1_tma_launch(Ctx &c, int cls, const void *maps, const Tvl1BlockedPlanes &B, int cur, int rows, int cols,
-                     const Tvl1Scalars &k, int iters, int num_sms, bool elect, bool tma_store) {
+                     const Tvl1Scalars &k, int iters, int num_sms) {
     const Tvl1State &so = B.s[cur ^ 1];
+    const TmaMaps *m = static_cast<const TmaMaps *>(maps);
     const TmaOutMaps *om = out_maps(maps);
-    // TMA-store path (the default): halo rounded up to a multiple of 4, so that every pass -- also the 6-iteration one that
-    // ends a 30-iteration warp -- takes the 64-wide boxes, the conflict-free LDS.128 fill and the TMA-store epilogue
-    // (a 6-pixel halo would need 72-wide boxes that fill registers through two-way conflicted LDS.64).  Without it: even
-    // halo >= iters (8-byte stores).
-    const int halo = tma_store ? ((iters + 3) & ~3) : ((iters + 1) & ~1);
+    // Halo rounded up to a multiple of 4: with iters <= TVL1_KMAX every halo and tile is then a multiple of 4, so every
+    // pass -- also the 6-iteration one that ends a 30-iteration warp -- takes the 64-wide boxes and the conflict-free
+    // LDS.128 fill.  Passes with an 8-pixel halo leave through the TMA-store epilogue, the others through 8-byte stores.
+    const int halo = (iters + 3) & ~3;
     const int tile = R - 2 * halo;
     const int tiles_x = div_up(cols, tile), tiles_y = div_up(rows, tile);
     const int ntiles = tiles_x * tiles_y;
     const int grid = ntiles < num_sms ? ntiles : num_sms;
     const double bytes = 64.0 * (double)rows * cols * iters;
-    const bool aligned = (halo & 3) == 0 && (tile & 3) == 0;  // every region origin is a multiple of 4
     // passes alternate their walking direction (see the kernel); `cur` flips with every pass and is 0 for the pass that
     // follows the warp kernel, which ended at the bottom of the image
     static const bool norev = getenv("B2F_DBG_TVL1_NOREV") != nullptr;
     const bool reverse = !norev && cur == 0;
-    const TmaMaps *m = static_cast<const TmaMaps *>(maps) + (aligned ? 1 : 0);
     // measurement aid (tools/gpu_probe_tile_cost.py): run fewer iterations than the geometry was laid out for, so the
     // per-tile cost of a pass (TMA wait, register fill, epilogue) separates from the per-iteration cost.  Results are
     // garbage with it; never set outside that probe.
     if (const char *dbg = getenv("B2F_DBG_TVL1_ITERS")) iters = atoi(dbg) < iters ? atoi(dbg) : iters;
-    if (aligned && halo == 8 && tma_store && !c.capturing && getenv("B2F_DBG_TVL1_CLOCKS")) {  // phase clocks of every tile
+    if (halo == 8 && !c.capturing && getenv("B2F_DBG_TVL1_CLOCKS")) {  // phase clocks of every tile
         static long long *buf = nullptr;
         static size_t cap = 0;
         const size_t need = (size_t)ntiles * 8;
@@ -1564,8 +544,8 @@ void tvl1_tma_launch(Ctx &c, int cls, const void *maps, const Tvl1BlockedPlanes 
             cudaMemcpyToSymbol(g_tvl1_clock_buf, &buf, sizeof(buf));
         }
         cudaMemsetAsync(buf, 0, need * sizeof(long long), c.stream);
-        B2F_LAUNCH(c, cls, bytes, (k_tvl1_blocked_tma<true, R, 3>), dim3(grid), dim3(NT), smem_tma_bytes(R), *m, so.u1,
-                   so.u2, so.p11, so.p12, so.p21, so.p22, rows, cols, k, iters, halo, tile, tiles_x, ntiles, nullptr, *om, 1);
+        B2F_LAUNCH(c, cls, bytes, k_tvl1_blocked_tma<true>, dim3(grid), dim3(NT), smem_tma_bytes(), *m, so.u1, so.u2,
+                   so.p11, so.p12, so.p21, so.p22, rows, cols, k, iters, halo, tile, tiles_x, ntiles, nullptr, *om, 1);
         cudaStreamSynchronize(c.stream);
         std::vector<long long> h(need);
         cudaMemcpy(h.data(), buf, need * sizeof(long long), cudaMemcpyDeviceToHost);
@@ -1582,158 +562,23 @@ void tvl1_tma_launch(Ctx &c, int cls, const void *maps, const Tvl1BlockedPlanes 
                 ph[2] / n, ph[3] / n, iters ? ph[3] / n / iters : 0.0, ph[4] / n, ngap ? ph[5] / ngap : 0.0);
         return;
     }
-    if (aligned)
-        B2F_LAUNCH(c, cls, bytes, (k_tvl1_blocked_tma<true, R>), dim3(grid), dim3(NT), smem_tma_bytes(R), *m, so.u1,
-                   so.u2, so.p11, so.p12, so.p21, so.p22, rows, cols, k, iters, halo, tile, tiles_x, ntiles, nullptr, *om,
-                   ((tma_store && halo == 8) ? 1 : 0) | (reverse ? 2 : 0));
-    else if (elect)
-        B2F_LAUNCH(c, cls, bytes, (k_tvl1_blocked_tma<true, TBOX_WIDE>), dim3(grid), dim3(NT),
-                   smem_tma_bytes(TBOX_WIDE), *m, so.u1, so.u2, so.p11, so.p12, so.p21, so.p22, rows, cols, k, iters,
-                   halo, tile, tiles_x, ntiles, nullptr, *om, 0);
-    else
-        B2F_LAUNCH(c, cls, bytes, (k_tvl1_blocked_tma<false, TBOX_WIDE>), dim3(grid), dim3(NT),
-                   smem_tma_bytes(TBOX_WIDE), *m, so.u1, so.u2, so.p11, so.p12, so.p21, so.p22, rows, cols, k, iters,
-                   halo, tile, tiles_x, ntiles, nullptr, *om, 0);
-}
-
-// Two-group (anti-phase) variant of the aligned kernel; halo rounded up to a multiple of 4 like the packed kernel.
-void tvl1_tma2g_launch(Ctx &c, int cls, const void *maps, const Tvl1BlockedPlanes &B, int cur, int rows, int cols,
-                       const Tvl1Scalars &k, int iters, int num_sms) {
-    const Tvl1State &so = B.s[cur ^ 1];
-    const int halo = (iters + 3) & ~3;
-    const int tile = R - 2 * halo;
-    const int tiles_x = div_up(cols, tile), tiles_y = div_up(rows, tile);
-    const int ntiles = tiles_x * tiles_y;
-    const int grid = ntiles < num_sms ? ntiles : num_sms;
-    const double bytes = 64.0 * (double)rows * cols * iters;
-    const TmaMaps *m = static_cast<const TmaMaps *>(maps) + 1;
-    B2F_LAUNCH(c, cls, bytes, (k_tvl1_blocked_tma<true, R, 1>), dim3(grid), dim3(NT), smem_tma_bytes(R, 1),
-               *m, so.u1, so.u2, so.p11, so.p12, so.p21, so.p22, rows, cols, k, iters, halo, tile, tiles_x, ntiles, nullptr,
-               *out_maps(maps), 0);
-}
-
-// Neighbour-synchronised variant of the aligned kernel (kernel_path 9).
-void tvl1_tmanb_launch(Ctx &c, int cls, const void *maps, const Tvl1BlockedPlanes &B, int cur, int rows, int cols,
-                       const Tvl1Scalars &k, int iters, int num_sms, bool tma_store) {
-    const Tvl1State &so = B.s[cur ^ 1];
-    const int halo = (iters + 3) & ~3;
-    const int tile = R - 2 * halo;
-    const int tiles_x = div_up(cols, tile), tiles_y = div_up(rows, tile);
-    const int ntiles = tiles_x * tiles_y;
-    const int grid = ntiles < num_sms ? ntiles : num_sms;
-    const double bytes = 64.0 * (double)rows * cols * iters;
-    const TmaMaps *m = static_cast<const TmaMaps *>(maps) + 1;
-    B2F_LAUNCH(c, cls, bytes, (k_tvl1_blocked_tma<true, R, 2>), dim3(grid), dim3(NT), smem_tma_bytes(R, 2), *m, so.u1,
-               so.u2, so.p11, so.p12, so.p21, so.p22, rows, cols, k, iters, halo, tile, tiles_x, ntiles, nullptr,
-               *out_maps(maps), (tma_store && halo == 8) ? 1 : 0);
-}
-
-// Row-skewed variant of the aligned kernel (kernel_path 12).
-void tvl1_tmasp_launch(Ctx &c, int cls, const void *maps, const Tvl1BlockedPlanes &B, int cur, int rows, int cols,
-                       const Tvl1Scalars &k, int iters, int num_sms, bool tma_store) {
-    const Tvl1State &so = B.s[cur ^ 1];
-    const int halo = (iters + 3) & ~3;
-    const int tile = R - 2 * halo;
-    const int tiles_x = div_up(cols, tile), tiles_y = div_up(rows, tile);
-    const int ntiles = tiles_x * tiles_y;
-    const int grid = ntiles < num_sms ? ntiles : num_sms;
-    const double bytes = 64.0 * (double)rows * cols * iters;
-    const TmaMaps *m = static_cast<const TmaMaps *>(maps) + 1;
-    B2F_LAUNCH(c, cls, bytes, (k_tvl1_blocked_tma<true, R, 4>), dim3(grid), dim3(NT), smem_tma_bytes(R, 4), *m, so.u1,
-               so.u2, so.p11, so.p12, so.p21, so.p22, rows, cols, k, iters, halo, tile, tiles_x, ntiles, nullptr,
-               *out_maps(maps), (tma_store && halo == 8) ? 1 : 0);
+    B2F_LAUNCH(c, cls, bytes, k_tvl1_blocked_tma<>, dim3(grid), dim3(NT), smem_tma_bytes(), *m, so.u1, so.u2, so.p11,
+               so.p12, so.p21, so.p22, rows, cols, k, iters, halo, tile, tiles_x, ntiles, nullptr, *om,
+               (halo == 8 ? 1 : 0) | (reverse ? 2 : 0));
 }
 
 // One pass whose iteration count (0..8; negative = skip the pass) is read from device memory at run time: fixed
 // geometry (8-pixel halo, 48-pixel tiles, 64-wide boxes) so the launch can sit in a CUDA graph's while-loop body.
 void tvl1_tma_launch_dev(Ctx &c, int cls, const void *maps, const Tvl1BlockedPlanes &B, int cur, int rows, int cols,
-                         const Tvl1Scalars &k, const int *iters_dev, int num_sms, bool tma_store) {
+                         const Tvl1Scalars &k, const int *iters_dev, int num_sms) {
     const Tvl1State &so = B.s[cur ^ 1];
     const int halo = 8, tile = R - 2 * halo;
     const int tiles_x = div_up(cols, tile), tiles_y = div_up(rows, tile);
     const int ntiles = tiles_x * tiles_y;
     const int grid = ntiles < num_sms ? ntiles : num_sms;
-    const TmaMaps *m = static_cast<const TmaMaps *>(maps) + 1;
-    B2F_LAUNCH(c, cls, 0.0, (k_tvl1_blocked_tma<true, R>), dim3(grid), dim3(NT), smem_tma_bytes(R), *m, so.u1, so.u2,
-               so.p11, so.p12, so.p21, so.p22, rows, cols, k, 0, halo, tile, tiles_x, ntiles, iters_dev, *out_maps(maps),
-               tma_store ? 1 : 0);
-}
-
-constexpr size_t smem_packed_bytes() { return sizeof(float) * (size_t)(N_IN * R * R) + sizeof(float4) * 4 * PEX_F4 + 64; }
-
-// halo rounded up to a multiple of 4 keeps every region origin 16-byte aligned (TMA box rule, vector stores)
-void tvl1_packed_launch(Ctx &c, int cls, const void *maps, const Tvl1BlockedPlanes &B, int cur, int rows, int cols,
-                        const Tvl1Scalars &k, int iters, int num_sms) {
-    const Tvl1State &so = B.s[cur ^ 1];
-    const int halo = (iters + 3) & ~3;
-    const int tile = R - 2 * halo;
-    const int tiles_x = div_up(cols, tile), tiles_y = div_up(rows, tile);
-    const int ntiles = tiles_x * tiles_y;
-    const int grid = ntiles < num_sms ? ntiles : num_sms;
-    const double bytes = 64.0 * (double)rows * cols * iters;
-    const TmaMaps *m = static_cast<const TmaMaps *>(maps) + 1;  // the 64-wide box descriptors
-    B2F_LAUNCH(c, cls, bytes, k_tvl1_packed_tma, dim3(grid), dim3(NT), smem_packed_bytes(), *m, so.u1, so.u2, so.p11,
-               so.p12, so.p21, so.p22, rows, cols, k, iters, halo, tile, tiles_x, ntiles);
-}
-
-constexpr size_t smem_cluster_bytes() {
-    return sizeof(float) * (size_t)(N_IN * R * R + 4 * EX_F) + sizeof(ClusterGhosts) + 64;
-}
-
-// Clusters that can be co-resident (GPC boundaries cap it below SMs / cluster size); cached per shape.
-static int cluster_max_active(int cx, int cy, int num_sms) {
-    static int cache[3][3] = {};
-    if (cache[cx][cy]) return cache[cx][cy];
-    cudaLaunchConfig_t cfg = {};
-    cfg.gridDim = dim3(cx * cy * (num_sms / (cx * cy)));
-    cfg.blockDim = dim3(NT);
-    cfg.dynamicSmemBytes = smem_cluster_bytes();
-    cudaLaunchAttribute at;
-    at.id = cudaLaunchAttributeClusterDimension;
-    at.val.clusterDim.x = cx * cy;
-    at.val.clusterDim.y = 1;
-    at.val.clusterDim.z = 1;
-    cfg.attrs = &at;
-    cfg.numAttrs = 1;
-    int n = 0;
-    if (cudaOccupancyMaxActiveClusters(&n, k_tvl1_cluster_tma, &cfg) != cudaSuccess || n <= 0) {
-        cudaGetLastError();
-        n = num_sms / (cx * cy);
-    }
-    cache[cx][cy] = n;
-    return n;
-}
-
-int tvl1_cluster_max_active(int cx, int cy, int num_sms) { return cluster_max_active(cx, cy, num_sms); }
-
-void tvl1_cluster_launch(Ctx &c, int cls, const void *maps, const Tvl1BlockedPlanes &B, int cur, int rows, int cols,
-                         const Tvl1Scalars &k, int iters, int num_sms, int cx, int cy) {
-    const Tvl1State &so = B.s[cur ^ 1];
-    const int halo = (iters + 3) & ~3;   // multiples of 4: 16-byte TMA box origins and vector stores
-    const int stile_x = R * cx - 2 * halo, stile_y = R * cy - 2 * halo;
-    const int stiles_x = div_up(cols, stile_x), stiles_y = div_up(rows, stile_y);
-    const int n_super = stiles_x * stiles_y;
-    const int max_cl = cluster_max_active(cx, cy, num_sms);
-    const int n_clusters = n_super < max_cl ? n_super : max_cl;
-    const double bytes = 64.0 * (double)rows * cols * iters;
-    const TmaMaps *m = static_cast<const TmaMaps *>(maps) + 1;  // 64-wide boxes
-    if (!c.ok()) return;
-    c.pre(cls, bytes);
-    cudaLaunchConfig_t cfg = {};
-    cfg.gridDim = dim3(n_clusters * cx * cy);
-    cfg.blockDim = dim3(NT);
-    cfg.dynamicSmemBytes = smem_cluster_bytes();
-    cfg.stream = c.stream;
-    cudaLaunchAttribute at;
-    at.id = cudaLaunchAttributeClusterDimension;
-    at.val.clusterDim.x = cx * cy;
-    at.val.clusterDim.y = 1;
-    at.val.clusterDim.z = 1;
-    cfg.attrs = &at;
-    cfg.numAttrs = 1;
-    c.check(cudaLaunchKernelEx(&cfg, k_tvl1_cluster_tma, *m, so.u1, so.u2, so.p11, so.p12, so.p21, so.p22, rows, cols, k,
-                               iters, halo, cx, cy, stile_x, stile_y, stiles_x, n_super));
-    c.post(cls);
+    const TmaMaps *m = static_cast<const TmaMaps *>(maps);
+    B2F_LAUNCH(c, cls, 0.0, k_tvl1_blocked_tma<>, dim3(grid), dim3(NT), smem_tma_bytes(), *m, so.u1, so.u2, so.p11,
+               so.p12, so.p21, so.p22, rows, cols, k, 0, halo, tile, tiles_x, ntiles, iters_dev, *out_maps(maps), 1);
 }
 
 cudaError_t tvl1_blocked_init() {
@@ -1744,32 +589,11 @@ cudaError_t tvl1_blocked_init() {
     if (dev >= 0 && dev < 64 && done[dev]) return cudaSuccess;
     e = cudaFuncSetAttribute(k_tvl1_blocked, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SMEM_BYTES);
     if (e == cudaSuccess)
-        e = cudaFuncSetAttribute(k_tvl1_blocked_tma<true, TBOX_WIDE>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                 (int)smem_tma_bytes(TBOX_WIDE));
+        e = cudaFuncSetAttribute(k_tvl1_blocked_tma<false>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                 (int)smem_tma_bytes());
     if (e == cudaSuccess)
-        e = cudaFuncSetAttribute(k_tvl1_blocked_tma<false, TBOX_WIDE>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                 (int)smem_tma_bytes(TBOX_WIDE));
-    if (e == cudaSuccess)
-        e = cudaFuncSetAttribute(k_tvl1_blocked_tma<true, R>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                 (int)smem_tma_bytes(R));
-    if (e == cudaSuccess)
-        e = cudaFuncSetAttribute(k_tvl1_blocked_tma<true, R, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                 (int)smem_tma_bytes(R, 1));
-    if (e == cudaSuccess)
-        e = cudaFuncSetAttribute(k_tvl1_blocked_tma<true, R, 2>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                 (int)smem_tma_bytes(R, 2));
-    if (e == cudaSuccess)
-        e = cudaFuncSetAttribute(k_tvl1_blocked_tma<true, R, 3>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                 (int)smem_tma_bytes(R));
-    if (e == cudaSuccess)
-        e = cudaFuncSetAttribute(k_tvl1_blocked_tma<true, R, 4>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                 (int)smem_tma_bytes(R, 4));
-    if (e == cudaSuccess)
-        e = cudaFuncSetAttribute(k_tvl1_packed_tma, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                 (int)smem_packed_bytes());
-    if (e == cudaSuccess)
-        e = cudaFuncSetAttribute(k_tvl1_cluster_tma, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                 (int)smem_cluster_bytes());
+        e = cudaFuncSetAttribute(k_tvl1_blocked_tma<true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                 (int)smem_tma_bytes());
     if (e == cudaSuccess && dev >= 0 && dev < 64) done[dev] = true;
     return e;
 }

@@ -45,32 +45,14 @@ void tvl1_blocked_launch(Ctx &c, int cls, const Tvl1BlockedPlanes &B, int cur, i
 
 
 // ---- persistent TMA variant ----
-// Opaque per-(level, direction) descriptor block (10 CUtensorMaps), built once per workspace.
+// Opaque per-(level, direction) descriptor block (10 input and 6 output CUtensorMaps), built once per workspace.
 size_t tvl1_tma_maps_bytes();
 bool tvl1_tma_build_maps(void *dst, const Tvl1BlockedPlanes &B, int cur, int rows, int cols);
 void tvl1_tma_launch(Ctx &c, int cls, const void *maps, const Tvl1BlockedPlanes &B, int cur, int rows, int cols,
-                     const Tvl1Scalars &k, int iters, int num_sms, bool elect = true, bool tma_store = false);
+                     const Tvl1Scalars &k, int iters, int num_sms);
 
 // Same kernel, iteration count read from device memory when the pass runs (device-side convergence loop).
 void tvl1_tma_launch_dev(Ctx &c, int cls, const void *maps, const Tvl1BlockedPlanes &B, int cur, int rows, int cols,
-                         const Tvl1Scalars &k, const int *iters_dev, int num_sms, bool tma_store);
-
-// Two-group variant: the two halves of the region run half an iteration apart (FP32-bound primal against SFU-bound dual).
-void tvl1_tmanb_launch(Ctx &c, int cls, const void *maps, const Tvl1BlockedPlanes &B, int cur, int rows, int cols,
-                       const Tvl1Scalars &k, int iters, int num_sms, bool tma_store);
-// Row-skewed variant: the thread's independent pixel row runs between a split-phase arrive and its wait.
-void tvl1_tmasp_launch(Ctx &c, int cls, const void *maps, const Tvl1BlockedPlanes &B, int cur, int rows, int cols,
-                       const Tvl1Scalars &k, int iters, int num_sms, bool tma_store);
-void tvl1_tma2g_launch(Ctx &c, int cls, const void *maps, const Tvl1BlockedPlanes &B, int cur, int rows, int cols,
-                       const Tvl1Scalars &k, int iters, int num_sms);
-
-// Paired-strip persistent TMA kernel (kernel_path 5); iters <= TVL1_KMAX.
-void tvl1_packed_launch(Ctx &c, int cls, const void *maps, const Tvl1BlockedPlanes &B, int cur, int rows, int cols,
-                        const Tvl1Scalars &k, int iters, int num_sms);
-
-// Thread-block-cluster variant: cx x cy CTAs (2x2 or 2x1) share one super-region through DSMEM ghost exchange.
-void tvl1_cluster_launch(Ctx &c, int cls, const void *maps, const Tvl1BlockedPlanes &B, int cur, int rows, int cols,
-                         const Tvl1Scalars &k, int iters, int num_sms, int cx, int cy);
-int tvl1_cluster_max_active(int cx, int cy, int num_sms);
+                         const Tvl1Scalars &k, const int *iters_dev, int num_sms);
 
 }  // namespace b2f

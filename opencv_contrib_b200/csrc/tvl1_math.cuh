@@ -80,64 +80,6 @@ __device__ __forceinline__ void tvl1_update_p(float taut, float ux, float uy, fl
     pb = __fmul_rn(__fmaf_rn(taut, uy, pb), inv);
 }
 
-// ---------------------------------------------------------------------------------------------
-// Two-pixel form (kernel_path 5): the same arithmetic on TWO independent pixels per call.  Hopper
-// has no packed FP32 instruction, so each lane is one scalar IEEE round-to-nearest operation in the
-// same order as the scalar functions above; results are bit-identical to them.
-// ---------------------------------------------------------------------------------------------
-typedef float2 f2;
-__device__ __forceinline__ f2 fma2(f2 a, f2 b, f2 c) {
-    return make_float2(__fmaf_rn(a.x, b.x, c.x), __fmaf_rn(a.y, b.y, c.y));
-}
-__device__ __forceinline__ f2 mul2(f2 a, f2 b) { return make_float2(__fmul_rn(a.x, b.x), __fmul_rn(a.y, b.y)); }
-__device__ __forceinline__ f2 add2(f2 a, f2 b) { return make_float2(__fadd_rn(a.x, b.x), __fadd_rn(a.y, b.y)); }
-__device__ __forceinline__ f2 sub2(f2 a, f2 b) { return make_float2(__fsub_rn(a.x, b.x), __fsub_rn(a.y, b.y)); }
-__device__ __forceinline__ f2 splat2(float v) { return make_float2(v, v); }
-
-// tvl1_update_u for two pixels.  ninv = -tvl1_inv_grad(grad): (-rho) * inv == rho * (-inv) bit for bit.
-__device__ __forceinline__ void tvl1_update_u_x2(const Tvl1Scalars &k, f2 Ix, f2 Iy, f2 ninv, f2 rho_c, f2 u1, f2 u2,
-                                                 f2 p11, f2 p11_l, f2 p12, f2 p12_u, f2 p21, f2 p21_l, f2 p22,
-                                                 f2 p22_u, f2 &u1n, f2 &u2n) {
-    const f2 rho = fma2(Iy, u2, fma2(Ix, u1, rho_c));
-    f2 fi = mul2(rho, ninv);
-    fi.x = fminf(fmaxf(fi.x, -k.l_t), k.l_t);
-    fi.y = fminf(fmaxf(fi.y, -k.l_t), k.l_t);
-    const f2 v1 = fma2(fi, Ix, u1);
-    const f2 v2 = fma2(fi, Iy, u2);
-    const f2 div1 = add2(sub2(p11, p11_l), sub2(p12, p12_u));
-    const f2 div2 = add2(sub2(p21, p21_l), sub2(p22, p22_u));
-    const f2 th = splat2(k.theta);
-    u1n = fma2(th, div1, v1);
-    u2n = fma2(th, div2, v2);
-}
-
-// tvl1_update_p2 for two pixels (the three MUFU per pixel stay scalar: there is no packed SFU op).
-__device__ __forceinline__ void tvl1_update_p2_x2(float taut, f2 ux1, f2 uy1, f2 ux2, f2 uy2, f2 &p11, f2 &p12,
-                                                  f2 &p21, f2 &p22) {
-    const f2 s1 = fma2(ux1, ux1, mul2(uy1, uy1));
-    const f2 s2 = fma2(ux2, ux2, mul2(uy2, uy2));
-    const f2 g1 = make_float2(sqrt_approx(s1.x), sqrt_approx(s1.y));
-    const f2 g2 = make_float2(sqrt_approx(s2.x), sqrt_approx(s2.y));
-    const f2 t = splat2(taut), one = splat2(1.0f);
-    const f2 a1 = fma2(t, g1, one);
-    const f2 a2 = fma2(t, g2, one);
-    const f2 m = mul2(a1, a2);
-    const f2 r = make_float2(rcp_approx(m.x), rcp_approx(m.y));
-    const f2 inv1 = mul2(r, a2), inv2 = mul2(r, a1);
-    p11 = mul2(fma2(t, ux1, p11), inv1);
-    p12 = mul2(fma2(t, uy1, p12), inv1);
-    p21 = mul2(fma2(t, ux2, p21), inv2);
-    p22 = mul2(fma2(t, uy2, p22), inv2);
-}
-
-// Keys bicubic kernel, a = -0.5 (tvl1flow.cu:89-104).
-__device__ __forceinline__ float bicubic_coeff(float x_) {
-    const float x = fabsf(x_);
-    if (x <= 1.0f) return x * x * (1.5f * x - 2.5f) + 1.0f;
-    if (x < 2.0f) return x * (x * (-0.5f * x + 2.5f) - 4.0f) + 2.0f;
-    return 0.0f;
-}
-
 #endif  // __CUDACC__
 
 }  // namespace b2f

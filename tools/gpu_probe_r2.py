@@ -9,7 +9,7 @@ dev = torch.device("cuda:0")
 I0, I1, gt = synth.make_pair(1080, 1920, seed=0, kind="smooth")
 d0, d1 = torch.from_numpy(I0).to(dev), torch.from_numpy(I1).to(dev)
 ref = None
-cases = [tuple(int(v) for v in (c.split(":") + ["0"])[:3]) for c in (sys.argv[1:] or ["0:8", "6:8", "7:8", "6:12", "7:12"])]
+cases = [tuple(int(v) for v in (c.split(":") + ["0"])[:3]) for c in (sys.argv[1:] or ["0:8", "0:12"])]
 for path, K, aux in cases:
     algs = [ocb.OpticalFlowDual_TVL1_create(nscales=5, warps=10, epsilon=0.0, iterations=30) for _ in range(4)]
     for a in algs:

@@ -5,7 +5,6 @@ mkdir -p gpurun_out
 timeout 60 tools/ubench/cond_graph_test > gpurun_out/r2_cond_graph.log 2>&1; cat gpurun_out/r2_cond_graph.log
 timeout 1500 python -m pytest tests/test_tvl1_gpu.py tests/test_farneback_gpu.py tests/test_adjacent_gpu.py -x -q -m gpu > gpurun_out/r2c_pytest.log 2>&1
 tail -8 gpurun_out/r2c_pytest.log
-timeout 600 python tools/gpu_probe_r2.py 0:8 6:8 7:8 0:12 > gpurun_out/r2c_probe.log 2>&1; cat gpurun_out/r2c_probe.log
 timeout 300 python tools/gpu_probe_farneback.py 2>&1 | tail -12 > gpurun_out/r2c_probe_farn.log; cat gpurun_out/r2c_probe_farn.log
 python - <<'PY' > gpurun_out/r2c_cluster_info.log 2>&1
 import ctypes as C, sys, os

@@ -1,8 +1,6 @@
 #!/bin/bash
-# fourth GPU call: 3-MUFU math restored, cluster wait at CTA scope: TV-L1 tests, path sweep, default bench line
+# fourth GPU call: 3-MUFU math restored: TV-L1 tests, default bench line
 mkdir -p gpurun_out
 timeout 900 python -m pytest tests/test_tvl1_gpu.py -x -q -m gpu > gpurun_out/r2d_pytest.log 2>&1; tail -4 gpurun_out/r2d_pytest.log
-timeout 600 python tools/gpu_probe_r2.py 0:8 6:8 7:8 6:10 6:12 7:12 > gpurun_out/r2d_probe.log 2>&1; cat gpurun_out/r2d_probe.log
-timeout 300 ncu --set full --clock-control none --import-source on --launch-count 1 -f --kernel-name regex:k_tvl1_cluster_tma --launch-skip 165 -o gpurun_out/prof_tvl1_cluster_r2b python tools/prof_one.py tvl1 8 1 6 > /dev/null 2>&1
 timeout 900 python bench.py --steps 5 --warmup 3 > gpurun_out/r2d_bench_default.json 2> gpurun_out/r2d_bench_default.err
 tail -c 1500 gpurun_out/r2d_bench_default.json; tail -5 gpurun_out/r2d_bench_default.err

@@ -1,7 +1,5 @@
 #!/bin/bash
-# fifth GPU call: cluster kernel with role bits, warp kernel variants, Farneback occupancy variants
+# fifth GPU call: Farneback occupancy variants, TV-L1 and Farneback tests
 mkdir -p gpurun_out
-timeout 240 python tools/gpu_cluster_sanity.py > gpurun_out/r2e_cluster_sanity.log 2>&1; tail -3 gpurun_out/r2e_cluster_sanity.log
-timeout 600 python tools/gpu_probe_r2.py 0:8:0 0:8:1 6:8:0 7:8:0 > gpurun_out/r2e_probe.log 2>&1; cat gpurun_out/r2e_probe.log
 timeout 300 python tools/gpu_probe_farn_r2.py 0 3 4 > gpurun_out/r2e_probe_farn.log 2>&1; cat gpurun_out/r2e_probe_farn.log
 timeout 600 python -m pytest tests/test_tvl1_gpu.py tests/test_farneback_gpu.py -x -q -m gpu > gpurun_out/r2e_pytest.log 2>&1; tail -3 gpurun_out/r2e_pytest.log

@@ -4,7 +4,6 @@
 mkdir -p gpurun_out
 timeout 2400 python -m pytest tests -x -q -m gpu > gpurun_out/r2f_pytest_all.log 2>&1; tail -6 gpurun_out/r2f_pytest_all.log
 timeout 600 python -c "import __graft_entry__ as g; g.smoke()" > gpurun_out/r2f_smoke.log 2>&1; tail -2 gpurun_out/r2f_smoke.log
-timeout 400 python tools/gpu_probe_r2.py 0:8:0 0:8:2 0:8:1 > gpurun_out/r2f_probe.log 2>&1; cat gpurun_out/r2f_probe.log
 timeout 300 python tools/gpu_probe_farn_r2.py 0 2 4 > gpurun_out/r2f_probe_farn.log 2>&1; cat gpurun_out/r2f_probe_farn.log
 timeout 900 python bench.py --steps 5 --warmup 3 > gpurun_out/r2f_bench_default.json 2> gpurun_out/r2f_bench_default.err
 tail -c 800 gpurun_out/r2f_bench_default.json; tail -3 gpurun_out/r2f_bench_default.err

@@ -1,6 +1,5 @@
 #!/bin/bash
-# sixteenth GPU call: TMA loads / stores issued by ten / six warps instead of one lane: bit-equality, clocks, timing
+# sixteenth GPU call: TMA loads / stores issued by ten / six warps instead of one lane: clocks, timing
 mkdir -p gpurun_out
-B2F_SKIP_CLUSTER=1 timeout 600 python -m pytest tests/test_tvl1_gpu.py -x -q -m gpu -k "bit_identical_to_unfused or cuda_semantics or convergence_loop" > gpurun_out/r2p_pytest.log 2>&1; tail -5 gpurun_out/r2p_pytest.log
 timeout 300 python tools/gpu_probe_tile_clocks.py 2>&1 | grep -E "iters 8" > gpurun_out/r2p_clocks.log; cat gpurun_out/r2p_clocks.log
 timeout 300 python tools/gpu_probe_r2.py 0:8:3 > gpurun_out/r2p_probe.log 2>&1; cat gpurun_out/r2p_probe.log

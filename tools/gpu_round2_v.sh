@@ -1,7 +1,6 @@
 #!/bin/bash
-# programmatic dependent launch for the TV-L1 schedule: correctness (TV-L1 + video + batch tests), A/B against B2F_PDL=0 on one box
+# programmatic dependent launch for the TV-L1 schedule: A/B against B2F_PDL=0 on one GPU
 mkdir -p gpurun_out
-B2F_SKIP_CLUSTER=1 timeout 900 python -m pytest tests/test_tvl1_gpu.py tests/test_adjacent_gpu.py tests/test_compat_gpu.py -x -q -m gpu > gpurun_out/r2v_pytest.log 2>&1; tail -4 gpurun_out/r2v_pytest.log
 for r in 1 2; do
   B2F_PDL=0 timeout 300 python tools/gpu_probe_r2.py 0:8:0 2>&1 | sed 's/^/pdl off  /'
   timeout 300 python tools/gpu_probe_r2.py 0:8:0 2>&1 | sed 's/^/pdl on   /'

@@ -1,7 +1,6 @@
 #!/bin/bash
 # alternating tile walking direction of the iteration passes (first region of a pass = data the previous kernel touched last): A/B on one box
 mkdir -p gpurun_out
-B2F_SKIP_CLUSTER=1 timeout 600 python -m pytest tests/test_tvl1_gpu.py -x -q -m gpu -k "bit_identical_to_unfused or cuda_semantics or 1080p" > gpurun_out/r2w_pytest.log 2>&1; tail -3 gpurun_out/r2w_pytest.log
 for r in 1 2; do
   B2F_DBG_TVL1_NOREV=1 timeout 300 python tools/gpu_probe_r2.py 0:8:0 2>&1 | sed 's/^/forward      /'
   timeout 300 python tools/gpu_probe_r2.py 0:8:0 2>&1 | sed 's/^/alternating  /'

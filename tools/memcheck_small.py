@@ -16,7 +16,6 @@ for name, alg, a, b in [
         ("brox-pp", ocb.BroxOpticalFlow_create(0.197, 50.0, 0.8, 2, 10, 3), f0, f1),
         ("brox-coop", ocb.BroxOpticalFlow_create(0.197, 50.0, 0.8, 3, 10, 5), f0, f1),
         ("brox-exact-rsqrt", ocb.BroxOpticalFlow_create(0.197, 50.0, 0.8, 2, 10, 4), f0, f1),
-        ("tvl1-skewed", ocb.OpticalFlowDual_TVL1_create(nscales=2, warps=2, epsilon=0.0, iterations=8), d0, d1),
         ("denselk", ocb.DensePyrLKOpticalFlow_create(maxLevel=2, iters=4), d0, d1),
         ("denselk-generic", ocb.DensePyrLKOpticalFlow_create(winSize=(9, 7), maxLevel=1, iters=3), d0, d1),
         ("denselk-even", ocb.DensePyrLKOpticalFlow_create(winSize=(4, 6), maxLevel=1, iters=3), d0, d1),
@@ -27,8 +26,6 @@ for name, alg, a, b in [
         alg.setEngineOption("kernel_path", 3)
     if name == "brox-exact-rsqrt":
         alg.setEngineOption("aux_path", 1)
-    if name == "tvl1-skewed":
-        alg.setEngineOption("kernel_path", 12)
     if len(sys.argv) > 1 and not any(name.startswith(a) for a in sys.argv[1:]):
         continue
     alg.setEngineOption("use_graph", 0)
