@@ -114,6 +114,26 @@ typedef struct b2f_denselk_params {
     int use_initial_flow; /* 0  */
 } b2f_denselk_params;
 
+/* cv::optflow::createOptFlow_DeepFlow (optflow.hpp; defaults of the OpticalFlowDeepFlow constructor,
+ * modules/optflow/src/deepflow.cpp:62-73).  Inputs 8UC1 or 32FC1 of equal size and type, output 32FC2; the caller's
+ * flow is never read (the reference discards it, deepflow.cpp:132,146), so the video front end's warm start is
+ * refused.  sigma, downscale_factor, alpha, delta, gamma and omega are the reference's float members: the
+ * engine rounds them to float.  The pre-smoothing kernel length floor(3 sigma) * 2 + 1 must be 3 (0 < sigma < 1).  The reference class
+ * does not override getDefaultName; b2f_default_name reports "DenseOpticalFlow.DeepFlow". */
+typedef struct b2f_deepflow_params {
+    double sigma;               /* 0.6  Gaussian pre-smoothing                        */
+    int min_size;               /* 25   stop the pyramid when a side is <= min_size   */
+    double downscale_factor;    /* 0.95 */
+    int fixed_point_iterations; /* 5    */
+    int sor_iterations;         /* 25   */
+    double alpha;               /* 1.0  smoothness (VariationalRefinement gets 4 alpha) */
+    double delta;               /* 0.5  colour constancy (gets delta / 3)             */
+    double gamma;               /* 5.0  gradient constancy (gets gamma / 3)           */
+    double omega;               /* 1.6  SOR relaxation                                */
+    int max_layers;             /* 200  levels below the source at most (buildPyramid's loop), so up to
+                                           max_layers + 1 levels; 0 = the source level only */
+} b2f_deepflow_params;
+
 typedef struct b2f_handle b2f_handle;
 
 /* ---- construction: replaces the static ::create() factories.  A NULL params pointer means
@@ -124,11 +144,13 @@ B2F_API void b2f_tvl1_default_params(b2f_tvl1_params *p);
 B2F_API void b2f_farneback_default_params(b2f_farneback_params *p);
 B2F_API void b2f_brox_default_params(b2f_brox_params *p);
 B2F_API void b2f_denselk_default_params(b2f_denselk_params *p);
+B2F_API void b2f_deepflow_default_params(b2f_deepflow_params *p);
 
 B2F_API int b2f_tvl1_create(const b2f_tvl1_params *p, b2f_handle **out);           /* src/tvl1flow.cpp:385-391 */
 B2F_API int b2f_farneback_create(const b2f_farneback_params *p, b2f_handle **out); /* src/farneback.cpp:484-489 */
 B2F_API int b2f_brox_create(const b2f_brox_params *p, b2f_handle **out);           /* src/brox.cpp:190-194 */
 B2F_API int b2f_denselk_create(const b2f_denselk_params *p, b2f_handle **out);     /* src/pyrlk.cpp:402-405 */
+B2F_API int b2f_deepflow_create(const b2f_deepflow_params *p, b2f_handle **out);   /* optflow deepflow.cpp:171-174 */
 B2F_API void b2f_destroy(b2f_handle *h);
 
 /* ---- getters/setters: replace getTau()/setTau() ... (cudaoptflow.hpp:158-177,233-243,261-283,
@@ -158,6 +180,9 @@ typedef enum b2f_param_id {
     /* DensePyrLK */
     B2F_LK_WIN_WIDTH = 400, B2F_LK_WIN_HEIGHT, B2F_LK_MAX_LEVEL, B2F_LK_ITERS,
     B2F_LK_USE_INITIAL_FLOW,
+    /* DeepFlow */
+    B2F_DEEP_SIGMA = 500, B2F_DEEP_MIN_SIZE, B2F_DEEP_DOWNSCALE_FACTOR, B2F_DEEP_FIXED_POINT_ITERATIONS,
+    B2F_DEEP_SOR_ITERATIONS, B2F_DEEP_ALPHA, B2F_DEEP_DELTA, B2F_DEEP_GAMMA, B2F_DEEP_OMEGA, B2F_DEEP_MAX_LAYERS,
     /* engine knobs (no reference counterpart) */
     B2F_ENGINE_FUSED_ITERS = 900, /* TV-L1: inner iterations fused per HBM pass (0 = auto)     */
     B2F_ENGINE_USE_GRAPH = 901,   /* capture the fixed schedule in a CUDA graph (default 1)    */
@@ -191,7 +216,9 @@ typedef enum b2f_param_id {
      * step runs (all of them on a level that fits one 64x64 region or with B2F_BROX_PATH_COOP; the last launch of an
      * inner step runs the remainder; 0 for B2F_BROX_PATH_HALF_SWEEP, whose launch is half an iteration; at most 255).
      * kernel_path 3 falls back to kernel_path 0 on levels whose regions are not co-resident or that need more than one
-     * solver launch per inner step; this says whether it did. */
+     * solver launch per inner step; this says whether it did.  DeepFlow: the SOR iterations each solver launch of the
+     * level runs (chosen from the level's shape; all of them on a level that fits one 64x64 region, which runs its
+     * fixed-point steps in one launch). */
     B2F_ENGINE_ACTIVE_PATH = 1000
 } b2f_param_id;
 

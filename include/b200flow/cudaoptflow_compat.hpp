@@ -253,6 +253,44 @@ public:
     }
 };
 
+/** cv::optflow::createOptFlow_DeepFlow (optflow.hpp; modules/optflow/src/deepflow.cpp) on the GPU.  The reference's
+ *  OpticalFlowDeepFlow is a CPU cv::DenseOpticalFlow with no accessors; this class takes the cv::cuda calling convention
+ *  (device images and a Stream) and names its accessors after the constructor's fields.  `flow` is written, never
+ *  read. */
+class DeepFlowOpticalFlow : public DenseOpticalFlow, protected impl::HandleOwner {
+public:
+    B2F_ACCESSOR(double, Sigma, B2F_DEEP_SIGMA)
+    B2F_ACCESSOR(int, MinSize, B2F_DEEP_MIN_SIZE)
+    B2F_ACCESSOR(double, DownscaleFactor, B2F_DEEP_DOWNSCALE_FACTOR)
+    B2F_ACCESSOR(int, FixedPointIterations, B2F_DEEP_FIXED_POINT_ITERATIONS)
+    B2F_ACCESSOR(int, SorIterations, B2F_DEEP_SOR_ITERATIONS)
+    B2F_ACCESSOR(double, Alpha, B2F_DEEP_ALPHA)
+    B2F_ACCESSOR(double, Delta, B2F_DEEP_DELTA)
+    B2F_ACCESSOR(double, Gamma, B2F_DEEP_GAMMA)
+    B2F_ACCESSOR(double, Omega, B2F_DEEP_OMEGA)
+    B2F_ACCESSOR(int, MaxLayers, B2F_DEEP_MAX_LAYERS)
+
+    void calc(InputArray I0, InputArray I1, InputOutputArray flow, Stream &stream = Stream::Null()) override {
+        run(I0, I1, flow, stream, false);
+    }
+    String getDefaultName() const override { return b2f_default_name(h_); }
+
+    static Ptr<DeepFlowOpticalFlow> create(double sigma = 0.6, int minSize = 25, double downscaleFactor = 0.95,
+                                           int fixedPointIterations = 5, int sorIterations = 25, double alpha = 1.0,
+                                           double delta = 0.5, double gamma = 5.0, double omega = 1.6,
+                                           int maxLayers = 200) {
+        b2f_deepflow_params p{sigma, minSize, downscaleFactor, fixedPointIterations, sorIterations, alpha, delta, gamma,
+                              omega, maxLayers};
+        auto o = detail::make<DeepFlowOpticalFlow>();
+        const int st = b2f_deepflow_create(&p, &o->h_);
+        if (st != B2F_OK) detail::fail(st, "DeepFlowOpticalFlow::create");
+        return o;
+    }
+};
+
+/** cv::optflow::createOptFlow_DeepFlow with the reference's defaults. */
+inline Ptr<DeepFlowOpticalFlow> createOptFlow_DeepFlow() { return DeepFlowOpticalFlow::create(); }
+
 #undef B2F_ACCESSOR
 
 /** cv::cuda::SparsePyrLKOpticalFlow (cudaoptflow.hpp:189-226), same signature as the reference's

@@ -17,10 +17,12 @@ from .cudaoptflow import (  # noqa: F401
     FarnebackOpticalFlow,
     BroxOpticalFlow,
     DensePyrLKOpticalFlow,
+    DeepFlowOpticalFlow,
     OpticalFlowDual_TVL1_create,
     FarnebackOpticalFlow_create,
     BroxOpticalFlow_create,
     DensePyrLKOpticalFlow_create,
+    createOptFlow_DeepFlow,
     SparsePyrLKOpticalFlow,
     SparsePyrLKOpticalFlow_create,
     OPTFLOW_USE_INITIAL_FLOW,

@@ -100,7 +100,8 @@ int b2f_video_create(b2f_handle *h, int rows, int cols, int type, int depth, int
             v->warm_param = B2F_FARN_FLAGS;
             v->warm_off = static_cast<double>(static_cast<int>(flags) & ~B2F_OPTFLOW_USE_INITIAL_FLOW);
             v->warm_on = static_cast<double>(static_cast<int>(flags) | B2F_OPTFLOW_USE_INITIAL_FLOW);
-        } else {  // Brox and DensePyrLK have no initial-flow path (brox.cpp:129-188, pyrlk.cpp:238-299)
+        } else {  // Brox, DensePyrLK and DeepFlow have no initial-flow path (brox.cpp:129-188, pyrlk.cpp:238-299,
+                  // deepflow.cpp:132,146)
             delete v;
             return B2F_BAD_ARG;
         }

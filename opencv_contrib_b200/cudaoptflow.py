@@ -267,6 +267,23 @@ _accessors(DensePyrLKOpticalFlow, "denselk", {
     "max_level": ("MaxLevel", int), "iters": ("NumIters", int), "use_initial_flow": ("UseInitialFlow", bool)})
 
 
+class DeepFlowOpticalFlow(DenseOpticalFlow):
+    """cv::optflow::createOptFlow_DeepFlow's OpticalFlowDeepFlow (modules/optflow/src/deepflow.cpp) on the GPU.  The
+    reference class has no getters or setters; these follow its constructor's field names.  The caller's flow is never
+    read."""
+
+    def getActivePath(self, level: int) -> int:
+        """SOR iterations per solver launch the last calc ran on pyramid level `level` (B2F_ENGINE_ACTIVE_PATH)."""
+        return int(self._get(PARAM["engine"]["active_path"] + level))
+
+
+_accessors(DeepFlowOpticalFlow, "deepflow", {
+    "sigma": ("Sigma", float), "min_size": ("MinSize", int), "downscale_factor": ("DownscaleFactor", float),
+    "fixed_point_iterations": ("FixedPointIterations", int), "sor_iterations": ("SorIterations", int),
+    "alpha": ("Alpha", float), "delta": ("Delta", float), "gamma": ("Gamma", float), "omega": ("Omega", float),
+    "max_layers": ("MaxLayers", int)})
+
+
 def _create(cls, fn_name: str, params):
     l = _lib.lib()
     h = C.c_void_p()
@@ -303,6 +320,15 @@ def DensePyrLKOpticalFlow_create(winSize=(13, 13), maxLevel=3, iters=30, useInit
     """cv::cuda::DensePyrLKOpticalFlow::create (cudaoptflow.hpp:245-249)."""
     p = _lib.b2f_denselk_params(winSize[0], winSize[1], maxLevel, iters, int(useInitialFlow))
     return _create(DensePyrLKOpticalFlow, "b2f_denselk_create", p)
+
+
+def createOptFlow_DeepFlow(sigma=0.6, minSize=25, downscaleFactor=0.95, fixedPointIterations=5, sorIterations=25,
+                           alpha=1.0, delta=0.5, gamma=5.0, omega=1.6, maxLayers=200):
+    """cv::optflow::createOptFlow_DeepFlow (optflow.hpp), with the OpticalFlowDeepFlow constructor's defaults
+    (deepflow.cpp:62-73) as arguments."""
+    p = _lib.b2f_deepflow_params(sigma, minSize, downscaleFactor, fixedPointIterations, sorIterations, alpha, delta,
+                                 gamma, omega, maxLayers)
+    return _create(DeepFlowOpticalFlow, "b2f_deepflow_create", p)
 
 
 def _sparse_image(t) -> b2f_image:
