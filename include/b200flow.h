@@ -134,6 +134,37 @@ typedef struct b2f_deepflow_params {
                                            max_layers + 1 levels; 0 = the source level only */
 } b2f_deepflow_params;
 
+/* cv::DISOpticalFlow (opencv's video module, dense inverse search).  Inputs 8UC1 of equal size (anything else:
+ * B2F_UNSUPPORTED_TYPE), output 32FC2.  With use_initial_flow the caller's 32FC2 flow is read as the initial flow
+ * (cv::DISOpticalFlow::calc reads a flow of the frame's size and type): it is resized (INTER_LINEAR) to the coarsest
+ * level times 1 / 2^coarsest, and there each patch starts from it or from zero flow, whichever has the lower SSD.  On a
+ * single-level pyramid (finest == coarsest == 0) this is cv2's rule bit for bit; on deeper pyramids cv2's rule has not
+ * been established and the engine's result differs from cv2's.  Without it the coarsest level starts from zero.  Spatial propagation follows OpenCV's OpenCL kernels (every
+ * patch row scanned, then every patch descends), not its CPU path, so with propagation on the result agrees with
+ * cv2.DISOpticalFlow statistically, not bit for bit.  Only patch_size 8 is built (all three presets use it); any other
+ * size, a stride outside 1..patch_size, a finest_scale outside 0..5, or a frame too small for finest_scale is refused
+ * with B2F_BAD_ARG.  The coarsest level is min(coarsest_scale, the automatic rule) (coarsest_scale -1: the automatic
+ * rule).  The refinement stage is VariationalRefinement with omega 1.6 and 5 SOR iterations, as DIS configures it.
+ * cv2 reports the default name "my_object" for this class; b2f_default_name reports the same. */
+typedef struct b2f_dis_params {
+    int finest_scale;                      /* 2 (MEDIUM: 1)                                    */
+    int coarsest_scale;                    /* -1 = automatic                                   */
+    int patch_size;                        /* 8                                                */
+    int patch_stride;                      /* 4 (MEDIUM: 3)                                    */
+    int grad_descent_iterations;           /* 16 (ULTRAFAST: 12, MEDIUM: 25)                   */
+    int variational_refinement_iterations; /* 5 (ULTRAFAST: 0)                                 */
+    double alpha;                          /* 20  refinement smoothness                        */
+    double delta;                          /* 5   refinement colour constancy                  */
+    double gamma;                          /* 10  refinement gradient constancy                */
+    double epsilon;                        /* 0.01 refinement robust-function epsilon          */
+    int use_mean_normalization;            /* 1 */
+    int use_spatial_propagation;           /* 1 */
+    int use_initial_flow;                  /* 0  read the caller's flow as the initial flow    */
+} b2f_dis_params;
+
+/* cv::DISOpticalFlow::PRESET_* */
+enum { B2F_DIS_PRESET_ULTRAFAST = 0, B2F_DIS_PRESET_FAST = 1, B2F_DIS_PRESET_MEDIUM = 2 };
+
 typedef struct b2f_handle b2f_handle;
 
 /* ---- construction: replaces the static ::create() factories.  A NULL params pointer means
@@ -145,12 +176,14 @@ B2F_API void b2f_farneback_default_params(b2f_farneback_params *p);
 B2F_API void b2f_brox_default_params(b2f_brox_params *p);
 B2F_API void b2f_denselk_default_params(b2f_denselk_params *p);
 B2F_API void b2f_deepflow_default_params(b2f_deepflow_params *p);
+B2F_API void b2f_dis_default_params(b2f_dis_params *p, int preset); /* DISOpticalFlow::create(preset) */
 
 B2F_API int b2f_tvl1_create(const b2f_tvl1_params *p, b2f_handle **out);           /* src/tvl1flow.cpp:385-391 */
 B2F_API int b2f_farneback_create(const b2f_farneback_params *p, b2f_handle **out); /* src/farneback.cpp:484-489 */
 B2F_API int b2f_brox_create(const b2f_brox_params *p, b2f_handle **out);           /* src/brox.cpp:190-194 */
 B2F_API int b2f_denselk_create(const b2f_denselk_params *p, b2f_handle **out);     /* src/pyrlk.cpp:402-405 */
 B2F_API int b2f_deepflow_create(const b2f_deepflow_params *p, b2f_handle **out);   /* optflow deepflow.cpp:171-174 */
+B2F_API int b2f_dis_create(const b2f_dis_params *p, b2f_handle **out);             /* NULL: the FAST preset */
 B2F_API void b2f_destroy(b2f_handle *h);
 
 /* ---- getters/setters: replace getTau()/setTau() ... (cudaoptflow.hpp:158-177,233-243,261-283,
@@ -183,6 +216,11 @@ typedef enum b2f_param_id {
     /* DeepFlow */
     B2F_DEEP_SIGMA = 500, B2F_DEEP_MIN_SIZE, B2F_DEEP_DOWNSCALE_FACTOR, B2F_DEEP_FIXED_POINT_ITERATIONS,
     B2F_DEEP_SOR_ITERATIONS, B2F_DEEP_ALPHA, B2F_DEEP_DELTA, B2F_DEEP_GAMMA, B2F_DEEP_OMEGA, B2F_DEEP_MAX_LAYERS,
+    /* DIS */
+    B2F_DIS_FINEST_SCALE = 600, B2F_DIS_COARSEST_SCALE, B2F_DIS_PATCH_SIZE, B2F_DIS_PATCH_STRIDE,
+    B2F_DIS_GRADIENT_DESCENT_ITERATIONS, B2F_DIS_VARIATIONAL_REFINEMENT_ITERATIONS, B2F_DIS_VARIATIONAL_REFINEMENT_ALPHA,
+    B2F_DIS_VARIATIONAL_REFINEMENT_DELTA, B2F_DIS_VARIATIONAL_REFINEMENT_GAMMA, B2F_DIS_VARIATIONAL_REFINEMENT_EPSILON,
+    B2F_DIS_USE_MEAN_NORMALIZATION, B2F_DIS_USE_SPATIAL_PROPAGATION, B2F_DIS_USE_INITIAL_FLOW,
     /* engine knobs (no reference counterpart) */
     B2F_ENGINE_FUSED_ITERS = 900, /* TV-L1: inner iterations fused per HBM pass (0 = auto)     */
     B2F_ENGINE_USE_GRAPH = 901,   /* capture the fixed schedule in a CUDA graph (default 1)    */
@@ -218,7 +256,8 @@ typedef enum b2f_param_id {
      * kernel_path 3 falls back to kernel_path 0 on levels whose regions are not co-resident or that need more than one
      * solver launch per inner step; this says whether it did.  DeepFlow: the SOR iterations each solver launch of the
      * level runs (chosen from the level's shape; all of them on a level that fits one 64x64 region, which runs its
-     * fixed-point steps in one launch). */
+     * fixed-point steps in one launch).  DIS (s = pyramid scale, finest_scale .. coarsest): bits 0-7 the refinement's SOR
+     * iterations per solver launch (0 without refinement), bits 8-23 the patch rows hs, bits 24-39 the patch columns ws. */
     B2F_ENGINE_ACTIVE_PATH = 1000
 } b2f_param_id;
 
@@ -345,7 +384,7 @@ B2F_API int b2f_interpolate_frames(const b2f_image *frame0, const b2f_image *fra
 
 /* ---- batched frame-pair front end for one GPU (SURVEY.md 8b / 8e): N engine handles on N streams, pairs dealt
  *      round robin -- the pattern of the reference's own multi-stream test (test/test_optflow.cpp:468-528).
- *      algo: 1 TV-L1, 2 Farneback, 3 Brox, 4 DensePyrLK; params: the matching b2f_*_params (NULL = defaults).
+ *      algo: 1 TV-L1, 2 Farneback, 3 Brox, 4 DensePyrLK, 5 DeepFlow, 6 DIS; params: the matching b2f_*_params (NULL = defaults).
  *      Sharding over GPUs / processes and the NCCL result gather stay with the caller's process framework
  *      (opencv_contrib_b200/batch.py over torch.distributed). ---- */
 typedef struct b2f_batch b2f_batch;

@@ -291,6 +291,40 @@ public:
 /** cv::optflow::createOptFlow_DeepFlow with the reference's defaults. */
 inline Ptr<DeepFlowOpticalFlow> createOptFlow_DeepFlow() { return DeepFlowOpticalFlow::create(); }
 
+/** cv::DISOpticalFlow (opencv's video module) on the GPU, with its accessors, in the cv::cuda calling convention.  u8
+ *  images; with UseInitialFlow `flow` is read as the initial flow (see b2f_dis_params).  Spatial propagation follows OpenCV's OpenCL kernels (see b2f_dis_params). */
+class DISOpticalFlow : public DenseOpticalFlow, protected impl::HandleOwner {
+public:
+    enum { PRESET_ULTRAFAST = B2F_DIS_PRESET_ULTRAFAST, PRESET_FAST = B2F_DIS_PRESET_FAST, PRESET_MEDIUM = B2F_DIS_PRESET_MEDIUM };
+    B2F_ACCESSOR(int, FinestScale, B2F_DIS_FINEST_SCALE)
+    B2F_ACCESSOR(int, CoarsestScale, B2F_DIS_COARSEST_SCALE)
+    B2F_ACCESSOR(int, PatchSize, B2F_DIS_PATCH_SIZE)
+    B2F_ACCESSOR(int, PatchStride, B2F_DIS_PATCH_STRIDE)
+    B2F_ACCESSOR(int, GradientDescentIterations, B2F_DIS_GRADIENT_DESCENT_ITERATIONS)
+    B2F_ACCESSOR(int, VariationalRefinementIterations, B2F_DIS_VARIATIONAL_REFINEMENT_ITERATIONS)
+    B2F_ACCESSOR(float, VariationalRefinementAlpha, B2F_DIS_VARIATIONAL_REFINEMENT_ALPHA)
+    B2F_ACCESSOR(float, VariationalRefinementDelta, B2F_DIS_VARIATIONAL_REFINEMENT_DELTA)
+    B2F_ACCESSOR(float, VariationalRefinementGamma, B2F_DIS_VARIATIONAL_REFINEMENT_GAMMA)
+    B2F_ACCESSOR(float, VariationalRefinementEpsilon, B2F_DIS_VARIATIONAL_REFINEMENT_EPSILON)
+    B2F_ACCESSOR(bool, UseMeanNormalization, B2F_DIS_USE_MEAN_NORMALIZATION)
+    B2F_ACCESSOR(bool, UseSpatialPropagation, B2F_DIS_USE_SPATIAL_PROPAGATION)
+    B2F_ACCESSOR(bool, UseInitialFlow, B2F_DIS_USE_INITIAL_FLOW)
+
+    void calc(InputArray I0, InputArray I1, InputOutputArray flow, Stream &stream = Stream::Null()) override {
+        run(I0, I1, flow, stream, getUseInitialFlow());
+    }
+    String getDefaultName() const override { return b2f_default_name(h_); }
+
+    static Ptr<DISOpticalFlow> create(int preset = PRESET_FAST) {
+        b2f_dis_params p;
+        b2f_dis_default_params(&p, preset);
+        auto o = detail::make<DISOpticalFlow>();
+        const int st = b2f_dis_create(&p, &o->h_);
+        if (st != B2F_OK) detail::fail(st, "DISOpticalFlow::create");
+        return o;
+    }
+};
+
 #undef B2F_ACCESSOR
 
 /** cv::cuda::SparsePyrLKOpticalFlow (cudaoptflow.hpp:189-226), same signature as the reference's

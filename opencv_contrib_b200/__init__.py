@@ -18,11 +18,16 @@ from .cudaoptflow import (  # noqa: F401
     BroxOpticalFlow,
     DensePyrLKOpticalFlow,
     DeepFlowOpticalFlow,
+    DISOpticalFlow,
     OpticalFlowDual_TVL1_create,
     FarnebackOpticalFlow_create,
     BroxOpticalFlow_create,
     DensePyrLKOpticalFlow_create,
     createOptFlow_DeepFlow,
+    DISOpticalFlow_create,
+    DISOPTICAL_FLOW_PRESET_ULTRAFAST,
+    DISOPTICAL_FLOW_PRESET_FAST,
+    DISOPTICAL_FLOW_PRESET_MEDIUM,
     SparsePyrLKOpticalFlow,
     SparsePyrLKOpticalFlow_create,
     OPTFLOW_USE_INITIAL_FLOW,

@@ -55,6 +55,14 @@ class b2f_deepflow_params(C.Structure):
                 ("delta", C.c_double), ("gamma", C.c_double), ("omega", C.c_double), ("max_layers", C.c_int)]
 
 
+class b2f_dis_params(C.Structure):
+    _fields_ = [("finest_scale", C.c_int), ("coarsest_scale", C.c_int), ("patch_size", C.c_int),
+                ("patch_stride", C.c_int), ("grad_descent_iterations", C.c_int),
+                ("variational_refinement_iterations", C.c_int), ("alpha", C.c_double), ("delta", C.c_double),
+                ("gamma", C.c_double), ("epsilon", C.c_double), ("use_mean_normalization", C.c_int),
+                ("use_spatial_propagation", C.c_int), ("use_initial_flow", C.c_int)]
+
+
 class b2f_sparselk_params(C.Structure):
     _fields_ = [("win_width", C.c_int), ("win_height", C.c_int), ("max_level", C.c_int), ("iters", C.c_int),
                 ("use_initial_flow", C.c_int)]
@@ -83,12 +91,14 @@ SYMBOLS = [
     ("b2f_brox_default_params", None, [C.POINTER(b2f_brox_params)]),
     ("b2f_denselk_default_params", None, [C.POINTER(b2f_denselk_params)]),
     ("b2f_deepflow_default_params", None, [C.POINTER(b2f_deepflow_params)]),
+    ("b2f_dis_default_params", None, [C.POINTER(b2f_dis_params), C.c_int]),
     ("b2f_tvl1_create", C.c_int, [C.POINTER(b2f_tvl1_params), C.POINTER(_H)]),
     ("b2f_median_blur_32f", C.c_int, [C.POINTER(b2f_image), C.POINTER(b2f_image), C.c_int, C.c_void_p]),
     ("b2f_farneback_create", C.c_int, [C.POINTER(b2f_farneback_params), C.POINTER(_H)]),
     ("b2f_brox_create", C.c_int, [C.POINTER(b2f_brox_params), C.POINTER(_H)]),
     ("b2f_denselk_create", C.c_int, [C.POINTER(b2f_denselk_params), C.POINTER(_H)]),
     ("b2f_deepflow_create", C.c_int, [C.POINTER(b2f_deepflow_params), C.POINTER(_H)]),
+    ("b2f_dis_create", C.c_int, [C.POINTER(b2f_dis_params), C.POINTER(_H)]),
     ("b2f_destroy", None, [_H]),
     ("b2f_set_param", C.c_int, [_H, C.c_int, C.c_double]),
     ("b2f_get_param", C.c_int, [_H, C.c_int, C.POINTER(C.c_double)]),
@@ -160,6 +170,9 @@ PARAM = {
     "denselk": dict(win_width=400, win_height=401, max_level=402, iters=403, use_initial_flow=404),
     "deepflow": dict(sigma=500, min_size=501, downscale_factor=502, fixed_point_iterations=503, sor_iterations=504,
                      alpha=505, delta=506, gamma=507, omega=508, max_layers=509),
+    "dis": dict(finest_scale=600, coarsest_scale=601, patch_size=602, patch_stride=603, grad_descent_iterations=604,
+                variational_refinement_iterations=605, alpha=606, delta=607, gamma=608, epsilon=609,
+                use_mean_normalization=610, use_spatial_propagation=611, use_initial_flow=612),
     "engine": dict(fused_iters=900, use_graph=901, kernel_path=902, aux_path=903, active_path=1000),
 }
 # b2f_tvl1_path flags (include/b200flow.h)

@@ -100,6 +100,10 @@ int b2f_video_create(b2f_handle *h, int rows, int cols, int type, int depth, int
             v->warm_param = B2F_FARN_FLAGS;
             v->warm_off = static_cast<double>(static_cast<int>(flags) & ~B2F_OPTFLOW_USE_INITIAL_FLOW);
             v->warm_on = static_cast<double>(static_cast<int>(flags) | B2F_OPTFLOW_USE_INITIAL_FLOW);
+        } else if (h->algo == b2f::ALGO_DIS) {
+            v->warm_param = B2F_DIS_USE_INITIAL_FLOW;
+            v->warm_on = 1;
+            v->warm_off = 0;
         } else {  // Brox, DensePyrLK and DeepFlow have no initial-flow path (brox.cpp:129-188, pyrlk.cpp:238-299,
                   // deepflow.cpp:132,146)
             delete v;

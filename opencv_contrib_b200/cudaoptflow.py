@@ -284,6 +284,34 @@ _accessors(DeepFlowOpticalFlow, "deepflow", {
     "max_layers": ("MaxLayers", int)})
 
 
+class DISOpticalFlow(DenseOpticalFlow):
+    """cv::DISOpticalFlow (opencv's video module) on the GPU, with cv2's accessor names.  Inputs are u8.  Spatial
+    propagation follows OpenCV's OpenCL kernels, so with it on the result agrees with cv2's CPU class statistically, not
+    bit for bit.  Only patch size 8 is built.  With setUseInitialFlow(True) the caller's flow is read as the initial
+    flow (see b2f_dis_params)."""
+
+    def _needs_initial_flow(self) -> bool:
+        return bool(self.getUseInitialFlow())
+
+    def getActivePath(self, level: int):
+        """(ws, hs, refinement SOR iterations per solver launch) the last calc ran on pyramid scale `level`
+        (B2F_ENGINE_ACTIVE_PATH)."""
+        v = int(self._get(PARAM["engine"]["active_path"] + level))
+        return v >> 24, (v >> 8) & 0xFFFF, v & 0xFF
+
+
+_accessors(DISOpticalFlow, "dis", {
+    "finest_scale": ("FinestScale", int), "coarsest_scale": ("CoarsestScale", int), "patch_size": ("PatchSize", int),
+    "patch_stride": ("PatchStride", int), "grad_descent_iterations": ("GradientDescentIterations", int),
+    "variational_refinement_iterations": ("VariationalRefinementIterations", int),
+    "alpha": ("VariationalRefinementAlpha", float), "delta": ("VariationalRefinementDelta", float),
+    "gamma": ("VariationalRefinementGamma", float), "epsilon": ("VariationalRefinementEpsilon", float),
+    "use_mean_normalization": ("UseMeanNormalization", bool),
+    "use_spatial_propagation": ("UseSpatialPropagation", bool), "use_initial_flow": ("UseInitialFlow", bool)})
+
+DISOPTICAL_FLOW_PRESET_ULTRAFAST, DISOPTICAL_FLOW_PRESET_FAST, DISOPTICAL_FLOW_PRESET_MEDIUM = 0, 1, 2
+
+
 def _create(cls, fn_name: str, params):
     l = _lib.lib()
     h = C.c_void_p()
@@ -329,6 +357,13 @@ def createOptFlow_DeepFlow(sigma=0.6, minSize=25, downscaleFactor=0.95, fixedPoi
     p = _lib.b2f_deepflow_params(sigma, minSize, downscaleFactor, fixedPointIterations, sorIterations, alpha, delta,
                                  gamma, omega, maxLayers)
     return _create(DeepFlowOpticalFlow, "b2f_deepflow_create", p)
+
+
+def DISOpticalFlow_create(preset=DISOPTICAL_FLOW_PRESET_FAST):
+    """cv::DISOpticalFlow::create(preset) (cv2.DISOpticalFlow_create)."""
+    p = _lib.b2f_dis_params()
+    _lib.lib().b2f_dis_default_params(C.byref(p), int(preset))
+    return _create(DISOpticalFlow, "b2f_dis_create", p)
 
 
 def _sparse_image(t) -> b2f_image:

@@ -1,7 +1,8 @@
 #!/usr/bin/env python
 """Twin of the reference's evaluation sample (modules/optflow/samples/optical_flow_evaluation.cpp):
 
-    python tools/flow_eval.py image1 image2 {tvl1,farneback,brox,denselk} [groundtruth.flo]
+    python tools/flow_eval.py image1 image2 {tvl1,farneback,brox,denselk,dis_ultrafast,dis_fast,dis_medium}
+                              [groundtruth.flo]
                               [-m endpoint|angular|angular-fixed] [-o out.flo]
 
 computes the flow between two images on the GPU, optionally writes it as a Middlebury .flo file and, given a
@@ -18,7 +19,8 @@ def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("image1")
     ap.add_argument("image2")
-    ap.add_argument("algorithm", choices=["tvl1", "farneback", "brox", "denselk"])
+    ap.add_argument("algorithm", choices=["tvl1", "farneback", "brox", "denselk", "dis_ultrafast", "dis_fast",
+                                                  "dis_medium"])
     ap.add_argument("groundtruth", nargs="?")
     ap.add_argument("-m", "--measure", default="endpoint", choices=["endpoint", "angular", "angular-fixed"])
     ap.add_argument("-o", "--out")
@@ -35,6 +37,11 @@ def main():
     if a.algorithm == "brox":
         alg = ocb.BroxOpticalFlow_create(0.197, 50.0, 0.8, 10, 77, 10)
         d1, d2 = (torch.from_numpy((x / np.float32(255)).astype(np.float32)).to(dev) for x in (i1, i2))
+    elif a.algorithm.startswith("dis_"):
+        alg = ocb.DISOpticalFlow_create({"dis_ultrafast": ocb.DISOPTICAL_FLOW_PRESET_ULTRAFAST,
+                                         "dis_fast": ocb.DISOPTICAL_FLOW_PRESET_FAST,
+                                         "dis_medium": ocb.DISOPTICAL_FLOW_PRESET_MEDIUM}[a.algorithm])
+        d1, d2 = torch.from_numpy(i1).to(dev), torch.from_numpy(i2).to(dev)
     else:
         alg = {"tvl1": ocb.OpticalFlowDual_TVL1_create, "farneback": ocb.FarnebackOpticalFlow_create,
                "denselk": ocb.DensePyrLKOpticalFlow_create}[a.algorithm]()
