@@ -744,7 +744,6 @@ struct BLevel {
 class BroxEngine : public b2f_handle {
 public:
     explicit BroxEngine(const b2f_brox_params &p) : P(p) { algo = ALGO_BROX; }
-    ~BroxEngine() override { destroy_graph(); }
     b2f_brox_params P;
 
     int calc(const b2f_image *I0, const b2f_image *I1, b2f_image *flow, cudaStream_t s) override;
@@ -775,21 +774,18 @@ private:
     unsigned *coop_barrier_ = nullptr;  // arrival counter of the cooperative level kernel (zeroed before every launch)
     int coop_max_blocks_[2] = {-1, -1}; // co-resident CTAs of k_brox_level_coop<aux_path == 1> on this device (0: unsupported)
     bool coop_ok(int blocks, bool exact_rsq);
-    // b2f_brox_path | iterations per solver launch << 8, per solved level: of the last calc (B2F_ENGINE_ACTIVE_PATH)
-    // and of the captured graph
-    std::vector<int> level_paths_, graph_level_paths_;
-    int num_sms_ = 0;       // SM count of this handle's device (launch-cost model of the fused solver)
     int final_ui_ = 0;      // which (u, v) buffer pair holds the result (fixed by the level count)
 
-    cudaGraphExec_t graph_exec_ = nullptr;
-    struct Key { int rows = 0, cols = 0; b2f_brox_params P{}; EngineKnobs knobs; void *base = nullptr; } key_;
-    uint64_t g_launches_ = 0, g_cls_launches_[B2F_MAX_KERNEL_CLASSES] = {};
-    double g_cls_bytes_[B2F_MAX_KERNEL_CLASSES] = {};
-    int g_iters_ = 0;
-    void destroy_graph() {
-        if (graph_exec_) cudaGraphExecDestroy(graph_exec_);
-        graph_exec_ = nullptr;
-    }
+    struct GraphKey {
+        int rows, cols;
+        b2f_brox_params P;
+        EngineKnobs knobs;
+        const void *base;
+        bool operator==(const GraphKey &o) const {
+            return rows == o.rows && cols == o.cols && same_params(P, o.P) && same_knobs(knobs, o.knobs) && base == o.base;
+        }
+    };
+    GraphCache<GraphKey> graph_;
 
     size_t layout(int rows, int cols, bool counting, Layout &L);
     cudaError_t ensure_workspace(int rows, int cols);
@@ -842,7 +838,7 @@ cudaError_t BroxEngine::ensure_workspace(int rows, int cols) {
         return cudaSuccess;
     Layout tmp;
     const size_t need = layout(rows, cols, true, tmp);
-    destroy_graph();
+    graph_.destroy();
     cudaError_t e = arena.reserve(need);
     if (e != cudaSuccess) return e;
     layout(rows, cols, false, L_);
@@ -853,15 +849,14 @@ bool BroxEngine::coop_ok(int blocks, bool exact_rsq) {
     int &max_blocks = coop_max_blocks_[exact_rsq];
     if (max_blocks < 0) {
         max_blocks = 0;
-        int dev = 0, coop = 0, sms = 0, per_sm = 0;
+        int dev = 0, coop = 0, per_sm = 0;
         const size_t smem = sizeof(float) * 10 * SR * SR;
         auto kern = exact_rsq ? k_brox_level_coop<true> : k_brox_level_coop<false>;
         if (cudaGetDevice(&dev) == cudaSuccess &&
             cudaDeviceGetAttribute(&coop, cudaDevAttrCooperativeLaunch, dev) == cudaSuccess && coop &&
-            cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev) == cudaSuccess &&
             cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) == cudaSuccess &&
             cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kern, S_THREADS, smem) == cudaSuccess)
-            max_blocks = per_sm * sms;
+            max_blocks = per_sm * sm_count();
         cudaGetLastError();
         if (getenv("B2F_BROX_NO_COOP")) max_blocks = 0;
     }
@@ -920,14 +915,6 @@ void BroxEngine::solve(Ctx &c) {
         // more CTAs).  Small and mid levels are latency-bound (one wave), so they take all iterations in
         // one launch; large levels keep the tile big.  Cost model in microseconds: fill ~3, half sweep
         // ~0.35, launch gap ~2, per wave of one CTA per SM.
-        if (!num_sms_) {
-            int dev = 0;
-            if (cudaGetDevice(&dev) != cudaSuccess ||
-                cudaDeviceGetAttribute(&num_sms_, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || num_sms_ <= 0) {
-                cudaGetLastError();
-                num_sms_ = 132;
-            }
-        }
         int it_best = 5;
         if (!single && knobs.fused_iters > 0) {
             it_best = knobs.fused_iters;
@@ -937,7 +924,7 @@ void BroxEngine::solve(Ctx &c) {
                 const int t = SR - 4 * cand;
                 if (t < 8) break;
                 const int launches = div_up(P.solver_iterations, cand);
-                const double waves = std::ceil((double)div_up(w, t) * div_up(h, t) / (double)num_sms_);
+                const double waves = std::ceil((double)div_up(w, t) * div_up(h, t) / (double)sm_count());
                 const double cost = launches * (waves * (3.0 + 0.7 * cand) + 2.0);
                 if (cost < best) {
                     best = cost;
@@ -968,7 +955,7 @@ void BroxEngine::solve(Ctx &c) {
             } else if (knobs.kernel_path == 2) {
                 path = B2F_BROX_PATH_SMEM;
             }
-            level_paths_[l] = path | std::min(per_launch, 255) << 8;
+            active_paths[l] = path | std::min(per_launch, 255) << 8;
         }
         if (use_coop) {
             c.check(cudaMemsetAsync(coop_barrier_, 0, sizeof(unsigned), c.stream));
@@ -1060,23 +1047,18 @@ int BroxEngine::calc(const b2f_image *I0, const b2f_image *I1, b2f_image *flow, 
         return B2F_BAD_ARG;
     const int rows = I0->rows, cols = I0->cols;
     Ctx c = make_ctx(s);
-    {
-        static bool attr_done[64] = {};
-        int dev = 0;
-        cudaGetDevice(&dev);
-        if (dev >= 0 && dev < 64 && !attr_done[dev]) {
-            c.check(cudaFuncSetAttribute(k_brox_sor_fused_pp, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                         (int)(sizeof(float) * 11 * SR * SR)));
-            c.check(cudaFuncSetAttribute(k_brox_sor_reg, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                         (int)(sizeof(float) * 10 * SR * SR)));
-            attr_done[dev] = c.ok();
-        }
-    }
+    static DeviceOnce attrs;
+    attrs.run(c, [&] {
+        c.check(cudaFuncSetAttribute(k_brox_sor_fused_pp, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                     (int)(sizeof(float) * 11 * SR * SR)));
+        c.check(cudaFuncSetAttribute(k_brox_sor_reg, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                     (int)(sizeof(float) * 10 * SR * SR)));
+    });
     c.check(ensure_workspace(rows, cols));
     if (!c.ok()) return finish(c, s);
     stats.levels = static_cast<int>(L_.levels.size());
     stats.iterations_run = 0;
-    level_paths_.assign(L_.levels.size(), 0);
+    active_paths.assign(L_.levels.size(), 0.0);
 
     const ImageView v0{I0->data, I0->step, rows, cols, I0->type};
     const ImageView v1{I1->data, I1->step, rows, cols, I1->type};
@@ -1085,49 +1067,7 @@ int BroxEngine::calc(const b2f_image *I0, const b2f_image *I1, b2f_image *flow, 
 
     const bool want_graph = knobs.use_graph && !profiling && s != nullptr;
     if (want_graph) {
-        const bool hit = graph_exec_ && key_.rows == rows && key_.cols == cols && same_params(key_.P, P) &&
-                         same_knobs(key_.knobs, knobs) && key_.base == L_.levels[0].I0.p;
-        if (!hit) {
-            destroy_graph();
-            cudaStream_t cs = nullptr;
-            c.check(cudaStreamCreateWithFlags(&cs, cudaStreamNonBlocking));
-            if (c.ok()) {
-                Ctx g = make_ctx(cs);
-                b2f_stats scratch = stats;
-                g.stats = &scratch;
-                g.capturing = true;
-                g.check(cudaStreamBeginCapture(cs, cudaStreamCaptureModeThreadLocal));
-                if (g.ok()) solve(g);
-                cudaGraph_t graph = nullptr;
-                g.check(cudaStreamEndCapture(cs, &graph));
-                if (g.ok() && graph) g.check(cudaGraphInstantiate(&graph_exec_, graph, 0));
-                if (graph) cudaGraphDestroy(graph);
-                cudaStreamDestroy(cs);
-                g_launches_ = scratch.launches - stats.launches;
-                for (int i = 0; i < B2F_MAX_KERNEL_CLASSES; ++i) {
-                    g_cls_launches_[i] = scratch.class_launches[i] - stats.class_launches[i];
-                    g_cls_bytes_[i] = scratch.class_bytes[i] - stats.class_bytes[i];
-                }
-                g_iters_ = scratch.iterations_run;
-                c.check(g.err);
-                if (c.ok()) {
-                    key_.rows = rows; key_.cols = cols; key_.P = P; key_.knobs = knobs; key_.base = L_.levels[0].I0.p;
-                    graph_level_paths_ = level_paths_;
-                } else {
-                    destroy_graph();
-                }
-            }
-        }
-        if (c.ok() && graph_exec_) {
-            c.check(cudaGraphLaunch(graph_exec_, s));
-            stats.launches += g_launches_;
-            for (int i = 0; i < B2F_MAX_KERNEL_CLASSES; ++i) {
-                stats.class_launches[i] += g_cls_launches_[i];
-                stats.class_bytes[i] += g_cls_bytes_[i];
-            }
-            stats.iterations_run = g_iters_;
-            level_paths_ = graph_level_paths_;
-        }
+        graph_.run(*this, c, s, GraphKey{rows, cols, P, knobs, L_.levels[0].I0.p}, [&](Ctx &g) { solve(g); });
     } else {
         solve(c);
     }
@@ -1156,12 +1096,7 @@ int BroxEngine::get_param(int id, double *v) const {
         case B2F_BROX_INNER_ITERATIONS: *v = P.inner_iterations; break;
         case B2F_BROX_OUTER_ITERATIONS: *v = P.outer_iterations; break;
         case B2F_BROX_SOLVER_ITERATIONS: *v = P.solver_iterations; break;
-        default:
-            if (id >= B2F_ENGINE_ACTIVE_PATH && id - B2F_ENGINE_ACTIVE_PATH < (int)level_paths_.size()) {
-                *v = level_paths_[id - B2F_ENGINE_ACTIVE_PATH];
-                break;
-            }
-            return B2F_BAD_ARG;
+        default: return B2F_BAD_ARG;
     }
     return B2F_OK;
 }

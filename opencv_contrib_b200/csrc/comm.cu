@@ -45,28 +45,28 @@ struct NcclApi {
 };
 
 NcclApi *nccl_api() {
-    static NcclApi api;
-    static bool tried = false;
-    if (tried) return api.ok ? &api : nullptr;
-    tried = true;
-    void *h = dlopen("libnccl.so.2", RTLD_NOW | RTLD_NOLOAD);  // the copy torch already loaded, if any
-    if (!h) h = dlopen("libnccl.so.2", RTLD_NOW | RTLD_GLOBAL);
-    if (!h) return nullptr;
-    api.lib = h;
-#define B2F_SYM(field, name) *reinterpret_cast<void **>(&api.field) = dlsym(h, name)
-    B2F_SYM(GetUniqueId, "ncclGetUniqueId");
-    B2F_SYM(CommInitRank, "ncclCommInitRank");
-    B2F_SYM(CommInitRankConfig, "ncclCommInitRankConfig");
-    B2F_SYM(CommDestroy, "ncclCommDestroy");
-    B2F_SYM(CommCount, "ncclCommCount");
-    B2F_SYM(CommUserRank, "ncclCommUserRank");
-    B2F_SYM(Send, "ncclSend");
-    B2F_SYM(Recv, "ncclRecv");
-    B2F_SYM(GroupStart, "ncclGroupStart");
-    B2F_SYM(GroupEnd, "ncclGroupEnd");
+    static NcclApi api = [] {  // a function-local static is initialised once, thread-safely
+        NcclApi a;
+        void *h = dlopen("libnccl.so.2", RTLD_NOW | RTLD_NOLOAD);  // the copy torch already loaded, if any
+        if (!h) h = dlopen("libnccl.so.2", RTLD_NOW | RTLD_GLOBAL);
+        if (!h) return a;
+        a.lib = h;
+#define B2F_SYM(field, name) *reinterpret_cast<void **>(&a.field) = dlsym(h, name)
+        B2F_SYM(GetUniqueId, "ncclGetUniqueId");
+        B2F_SYM(CommInitRank, "ncclCommInitRank");
+        B2F_SYM(CommInitRankConfig, "ncclCommInitRankConfig");
+        B2F_SYM(CommDestroy, "ncclCommDestroy");
+        B2F_SYM(CommCount, "ncclCommCount");
+        B2F_SYM(CommUserRank, "ncclCommUserRank");
+        B2F_SYM(Send, "ncclSend");
+        B2F_SYM(Recv, "ncclRecv");
+        B2F_SYM(GroupStart, "ncclGroupStart");
+        B2F_SYM(GroupEnd, "ncclGroupEnd");
 #undef B2F_SYM
-    api.ok = api.GetUniqueId && api.CommInitRank && api.CommDestroy && api.CommCount && api.CommUserRank && api.Send &&
-             api.Recv && api.GroupStart && api.GroupEnd;
+        a.ok = a.GetUniqueId && a.CommInitRank && a.CommDestroy && a.CommCount && a.CommUserRank && a.Send && a.Recv &&
+               a.GroupStart && a.GroupEnd;
+        return a;
+    }();
     return api.ok ? &api : nullptr;
 }
 

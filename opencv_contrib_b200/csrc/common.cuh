@@ -13,6 +13,7 @@
 #include <stdint.h>
 #include <stddef.h>
 #include <float.h>
+#include <atomic>
 #include <vector>
 #include <string>
 
@@ -222,6 +223,14 @@ struct b2f_handle {
     // statistics that live on the device until the caller's stream has been synchronised (b2f_get_stats calls this)
     virtual void refresh_stats() {}
 
+    // What the last calc ran on each solved level, finest first: b2f_get_param answers B2F_ENGINE_ACTIVE_PATH +
+    // active_path_first + i with active_paths[i].  Engines fill it in their schedule; a graph replay restores it.
+    std::vector<double> active_paths;
+    int active_path_first = 0;
+    // SM count of the handle's device, queried once (132, the H100 SXM's, when the query fails)
+    int sm_count();
+    int sm_count_ = 0;
+
     b2f::Ctx make_ctx(cudaStream_t s);
     int finish(b2f::Ctx &ctx, cudaStream_t s);  // maps ctx.err -> status, NULL-stream sync
     void collect_profile();
@@ -230,23 +239,66 @@ struct b2f_handle {
 namespace b2f {
 
 // ---------------------------------------------------------------------------------------------
-// CUDA-graph cache of a fixed launch schedule (one per handle).  capture() records whatever `body` launches
-// through the Ctx it is given -- on a private capture stream -- and remembers the launch / byte accounting, so a
-// replay updates b2f_stats exactly like the eager path would.
+// Per-device one-time setup (kernel attributes) that any host thread may reach first.  run() calls `init`, which
+// reports through c.check, unless it already succeeded on the current device; a failure is retried by the next call.
 // ---------------------------------------------------------------------------------------------
-struct GraphCache {
-    cudaGraphExec_t exec = nullptr;
-    uint64_t launches = 0;
-    uint64_t class_launches[B2F_MAX_KERNEL_CLASSES] = {};
-    double class_bytes[B2F_MAX_KERNEL_CLASSES] = {};
-    int iterations = 0;
+class DeviceOnce {
+public:
+    template <class Init>
+    void run(Ctx &c, Init &&init) {
+        int dev = -1;
+        c.check(cudaGetDevice(&dev));
+        if (!c.ok()) return;
+        const bool tracked = dev >= 0 && dev < kMaxDevices;
+        if (tracked && done_[dev].load(std::memory_order_acquire)) return;
+        init();
+        if (tracked && c.ok()) done_[dev].store(true, std::memory_order_release);
+    }
+
+private:
+    static constexpr int kMaxDevices = 64;
+    std::atomic<bool> done_[kMaxDevices] = {};
+};
+
+// ---------------------------------------------------------------------------------------------
+// CUDA-graph cache of a fixed launch schedule (one per handle).  run() replays the graph when `key` equals the key it
+// was captured under.  Otherwise it records whatever `body` launches through the Ctx it is given -- on a private
+// capture stream -- and keeps the graph and the key only when the capture succeeded.  The key names everything the
+// schedule bakes in, the arena base included.  The capture's launch / byte accounting and the handle's active paths are
+// remembered, so a replay updates b2f_stats and active_paths exactly like the eager path would.
+// ---------------------------------------------------------------------------------------------
+template <class Key>
+class GraphCache {
+public:
     ~GraphCache() { destroy(); }
     void destroy() {
-        if (exec) cudaGraphExecDestroy(exec);
-        exec = nullptr;
+        if (exec_) cudaGraphExecDestroy(exec_);
+        exec_ = nullptr;
     }
+    // true when the graph ran on `s`; the active paths are restored only then
     template <class Body>
-    void capture(b2f_handle &h, Ctx &c, Body &&body) {
+    bool run(b2f_handle &h, Ctx &c, cudaStream_t s, const Key &key, Body &&body) {
+        if (!c.ok()) return false;
+        if (!exec_ || !(key_ == key)) {
+            capture(h, c, body);
+            if (!c.ok()) return false;
+            key_ = key;
+        }
+        c.check(cudaGraphLaunch(exec_, s));
+        h.stats.launches += launches_;
+        for (int i = 0; i < B2F_MAX_KERNEL_CLASSES; ++i) {
+            h.stats.class_launches[i] += class_launches_[i];
+            h.stats.class_bytes[i] += class_bytes_[i];
+        }
+        h.stats.iterations_run = iterations_;
+        if (!c.ok()) return false;
+        h.active_paths = paths_;
+        return true;
+    }
+
+private:
+    template <class Body>
+    void capture(b2f_handle &h, Ctx &c, Body &body) {
         destroy();
         cudaStream_t cs = nullptr;
         c.check(cudaStreamCreateWithFlags(&cs, cudaStreamNonBlocking));
@@ -261,28 +313,27 @@ struct GraphCache {
         if (g.ok()) body(g);
         cudaGraph_t graph = nullptr;
         g.check(cudaStreamEndCapture(cs, &graph));
-        if (g.ok() && graph) g.check(cudaGraphInstantiate(&exec, graph, 0));
+        if (g.ok() && graph) g.check(cudaGraphInstantiate(&exec_, graph, 0));
         if (graph) cudaGraphDestroy(graph);
         cudaStreamDestroy(cs);
-        launches = scratch.launches - h.stats.launches;
+        launches_ = scratch.launches - h.stats.launches;
         for (int i = 0; i < B2F_MAX_KERNEL_CLASSES; ++i) {
-            class_launches[i] = scratch.class_launches[i] - h.stats.class_launches[i];
-            class_bytes[i] = scratch.class_bytes[i] - h.stats.class_bytes[i];
+            class_launches_[i] = scratch.class_launches[i] - h.stats.class_launches[i];
+            class_bytes_[i] = scratch.class_bytes[i] - h.stats.class_bytes[i];
         }
-        iterations = scratch.iterations_run;
+        iterations_ = scratch.iterations_run;
+        paths_ = h.active_paths;
         c.check(g.err);
         if (!c.ok()) destroy();
     }
-    void replay(b2f_handle &h, Ctx &c, cudaStream_t s) {
-        if (!c.ok() || !exec) return;
-        c.check(cudaGraphLaunch(exec, s));
-        h.stats.launches += launches;
-        for (int i = 0; i < B2F_MAX_KERNEL_CLASSES; ++i) {
-            h.stats.class_launches[i] += class_launches[i];
-            h.stats.class_bytes[i] += class_bytes[i];
-        }
-        h.stats.iterations_run = iterations;
-    }
+
+    cudaGraphExec_t exec_ = nullptr;
+    Key key_{};
+    uint64_t launches_ = 0;
+    uint64_t class_launches_[B2F_MAX_KERNEL_CLASSES] = {};
+    double class_bytes_[B2F_MAX_KERNEL_CLASSES] = {};
+    int iterations_ = 0;
+    std::vector<double> paths_;
 };
 
 // ---------------------------------------------------------------------------------------------

@@ -83,10 +83,15 @@ private:
         float *shared[S_COUNT] = {};
     };
     Layout L_;
-    GraphCache graph_;
-    struct Key { int rows = 0, cols = 0; b2f_deepflow_params P{}; int use_graph = 1; void *base = nullptr; } key_;
-    std::vector<int> level_paths_, graph_level_paths_;  // SOR iterations per solver launch, per level
-    int num_sms_ = 0;
+    struct GraphKey {  // the schedule reads no knob
+        int rows, cols;
+        b2f_deepflow_params P;
+        const void *base;
+        bool operator==(const GraphKey &o) const {
+            return rows == o.rows && cols == o.cols && same_params(P, o.P) && base == o.base;
+        }
+    };
+    GraphCache<GraphKey> graph_;
     int final_ui_ = 0;
 
     size_t layout(int rows, int cols, bool counting, Layout &L);
@@ -164,8 +169,8 @@ void DeepFlowEngine::solve(Ctx &c) {
         T.du = sp(S_DU, w); T.dv = sp(S_DV, w);
         T.a12 = sp(S_A12, w); T.b1 = sp(S_B1, w); T.b2 = sp(S_B2, w);
         T.den_u = sp(S_DENU, w); T.den_v = sp(S_DENV, w); T.wr = sp(S_WR, w); T.wd = sp(S_WD, w);
-        const int it = variational_iters_per_launch(P.sor_iterations, h, w, num_sms_);
-        level_paths_[l] = it;
+        const int it = variational_iters_per_launch(P.sor_iterations, h, w, sm_count());
+        active_paths[l] = it;  // SOR iterations per solver launch
         variational_level(c, T, lv.I0, lv.I1, sp(S_AVG, w), sp(S_DUN, w), sp(S_DVN, w), h, w, k, P.fixed_point_iterations,
                           P.sor_iterations, it, CLS_SOR, CLS_TERMS, CLS_DERIV, CLS_PYR);
         if (l > 0) {
@@ -195,25 +200,16 @@ int DeepFlowEngine::calc(const b2f_image *I0, const b2f_image *I1, b2f_image *fl
     if (I0->step < (size_t)I0->cols * esz || I1->step < (size_t)I1->cols * esz || !flow_step_ok(flow)) return B2F_BAD_ARG;
     const int rows = I0->rows, cols = I0->cols;
     Ctx c = make_ctx(s);
-    {
-        static bool attr_done[64] = {};
-        int dev = 0;
-        cudaGetDevice(&dev);
-        if (dev >= 0 && dev < 64 && !attr_done[dev]) {
-            c.check(cudaFuncSetAttribute(k_df_sor, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                         (int)(sizeof(float) * SOR_PLANES * SR * SR)));
-            attr_done[dev] = c.ok();
-        }
-        if (!num_sms_ && (cudaDeviceGetAttribute(&num_sms_, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || num_sms_ <= 0)) {
-            cudaGetLastError();
-            num_sms_ = 132;
-        }
-    }
+    static DeviceOnce attrs;
+    attrs.run(c, [&] {
+        c.check(cudaFuncSetAttribute(k_df_sor, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                     (int)(sizeof(float) * SOR_PLANES * SR * SR)));
+    });
     c.check(ensure_workspace(rows, cols));
     if (!c.ok()) return finish(c, s);
     stats.levels = static_cast<int>(L_.levels.size());
     stats.iterations_run = 0;
-    level_paths_.assign(L_.levels.size(), 0);
+    active_paths.assign(L_.levels.size(), 0.0);
 
     const ImageView vf = flow_view(flow, rows, cols);
     {
@@ -235,17 +231,7 @@ int DeepFlowEngine::calc(const b2f_image *I0, const b2f_image *I1, b2f_image *fl
 
     const bool want_graph = knobs.use_graph && !profiling && s != nullptr;
     if (want_graph) {
-        const bool hit = graph_.exec && key_.rows == rows && key_.cols == cols && same_params(key_.P, P) &&
-                         key_.base == L_.levels[0].I0.p;
-        if (!hit) {
-            graph_.capture(*this, c, [&](Ctx &g) { solve(g); });
-            if (c.ok()) {
-                key_.rows = rows; key_.cols = cols; key_.P = P; key_.base = L_.levels[0].I0.p;
-                graph_level_paths_ = level_paths_;
-            }
-        }
-        graph_.replay(*this, c, s);
-        level_paths_ = graph_level_paths_;
+        graph_.run(*this, c, s, GraphKey{rows, cols, P, L_.levels[0].I0.p}, [&](Ctx &g) { solve(g); });
     } else {
         solve(c);
     }
@@ -282,12 +268,7 @@ int DeepFlowEngine::get_param(int id, double *v) const {
         case B2F_DEEP_GAMMA: *v = P.gamma; break;
         case B2F_DEEP_OMEGA: *v = P.omega; break;
         case B2F_DEEP_MAX_LAYERS: *v = P.max_layers; break;
-        default:
-            if (id >= B2F_ENGINE_ACTIVE_PATH && id - B2F_ENGINE_ACTIVE_PATH < (int)level_paths_.size()) {
-                *v = level_paths_[id - B2F_ENGINE_ACTIVE_PATH];
-                break;
-            }
-            return B2F_BAD_ARG;
+        default: return B2F_BAD_ARG;
     }
     return B2F_OK;
 }

@@ -406,10 +406,15 @@ private:
         Plane out_u{}, out_v{};
     };
     Layout L_;
-    GraphCache graph_;
-    struct Key { int rows = 0, cols = 0; b2f_dis_params P{}; void *base = nullptr; } key_;
-    std::vector<double> level_paths_, graph_level_paths_;  // per level, finest first
-    int num_sms_ = 0;
+    struct GraphKey {  // the schedule reads no knob
+        int rows, cols;
+        b2f_dis_params P;
+        const void *base;
+        bool operator==(const GraphKey &o) const {
+            return rows == o.rows && cols == o.cols && same_params(P, o.P) && base == o.base;
+        }
+    };
+    GraphCache<GraphKey> graph_;
 
     std::vector<std::pair<int, int>> level_sizes(int rows, int cols) const;
     size_t layout(int rows, int cols, bool counting, Layout &L);
@@ -541,13 +546,13 @@ void DISEngine::solve(Ctx &c) {
             R.du = sp(S_DU, w); R.dv = sp(S_DV, w);
             R.a12 = sp(S_A12, w); R.b1 = sp(S_B1, w); R.b2 = sp(S_B2, w);
             R.den_u = sp(S_DENU, w); R.den_v = sp(S_DENV, w); R.wr = sp(S_WR, w); R.wd = sp(S_WD, w);
-            it = variational_iters_per_launch(REFINE_SOR_ITERATIONS, h, w, num_sms_);
+            it = variational_iters_per_launch(REFINE_SOR_ITERATIONS, h, w, sm_count());
             variational_level(c, R, lv.I0, lv.I1, sp(S_AVG, w), sp(S_DUN, w), sp(S_DVN, w), h, w, k,
                               P.variational_refinement_iterations, REFINE_SOR_ITERATIONS, it, DCLS_REFINE, DCLS_REFINE,
                               DCLS_REFINE, DCLS_REFINE);
         }
         // bits 0-7: refinement SOR iterations per solver launch; bits 8-23: hs; 24-39: ws
-        level_paths_[l] = (double)it + 256.0 * ((double)hs + 65536.0 * (double)ws);
+        active_paths[l] = (double)it + 256.0 * ((double)hs + 65536.0 * (double)ws);
         if (l > 0) {
             const DLevel &nx = L_.levels[l - 1];
             Plane nu = sp(ui ? S_U : S_UN, nx.cols), nv = sp(ui ? S_V : S_VN, nx.cols);
@@ -578,25 +583,17 @@ int DISEngine::calc(const b2f_image *I0, const b2f_image *I1, b2f_image *flow, c
     const int rows = I0->rows, cols = I0->cols;
     if (level_sizes(rows, cols).empty()) return B2F_BAD_ARG;
     Ctx c = make_ctx(s);
-    {
-        static bool attr_done[64] = {};
-        int dev = 0;
-        cudaGetDevice(&dev);
-        if (dev >= 0 && dev < 64 && !attr_done[dev]) {
-            c.check(cudaFuncSetAttribute(k_df_sor, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                         (int)(sizeof(float) * SOR_PLANES * SR * SR)));
-            attr_done[dev] = c.ok();
-        }
-        if (!num_sms_ && (cudaDeviceGetAttribute(&num_sms_, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || num_sms_ <= 0)) {
-            cudaGetLastError();
-            num_sms_ = 132;
-        }
-    }
+    static DeviceOnce attrs;
+    attrs.run(c, [&] {
+        c.check(cudaFuncSetAttribute(k_df_sor, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                     (int)(sizeof(float) * SOR_PLANES * SR * SR)));
+    });
     c.check(ensure_workspace(rows, cols));
     if (!c.ok()) return finish(c, s);
     stats.levels = static_cast<int>(L_.levels.size());
     stats.iterations_run = 0;
-    level_paths_.assign(L_.levels.size(), 0.0);
+    active_paths.assign(L_.levels.size(), 0.0);  // level l is pyramid scale finest_scale + l
+    active_path_first = P.finest_scale;
 
     const ImageView vf = flow_view(flow, rows, cols);
     if (P.use_initial_flow) split_flow(c, DCLS_PYR, vf, L_.out_u, L_.out_v);  // read before the graph: the caller's buffer
@@ -609,17 +606,7 @@ int DISEngine::calc(const b2f_image *I0, const b2f_image *I1, b2f_image *flow, c
     }
     const bool want_graph = knobs.use_graph && !profiling && s != nullptr;
     if (want_graph) {
-        const bool hit = graph_.exec && key_.rows == rows && key_.cols == cols && same_params(key_.P, P) &&
-                         key_.base == L_.levels[0].I0.p;
-        if (!hit) {
-            graph_.capture(*this, c, [&](Ctx &g) { solve(g); });
-            if (c.ok()) {
-                key_.rows = rows; key_.cols = cols; key_.P = P; key_.base = L_.levels[0].I0.p;
-                graph_level_paths_ = level_paths_;
-            }
-        }
-        graph_.replay(*this, c, s);
-        level_paths_ = graph_level_paths_;
+        graph_.run(*this, c, s, GraphKey{rows, cols, P, L_.levels[0].I0.p}, [&](Ctx &g) { solve(g); });
     } else {
         solve(c);
     }
@@ -662,15 +649,7 @@ int DISEngine::get_param(int id, double *v) const {
         case B2F_DIS_USE_MEAN_NORMALIZATION: *v = P.use_mean_normalization; break;
         case B2F_DIS_USE_SPATIAL_PROPAGATION: *v = P.use_spatial_propagation; break;
         case B2F_DIS_USE_INITIAL_FLOW: *v = P.use_initial_flow; break;
-        default: {
-            // B2F_ENGINE_ACTIVE_PATH + s for pyramid scale s (0 = full size) of the last calc
-            const int s = id - B2F_ENGINE_ACTIVE_PATH - P.finest_scale;
-            if (id >= B2F_ENGINE_ACTIVE_PATH && s >= 0 && s < (int)level_paths_.size()) {
-                *v = level_paths_[s];
-                break;
-            }
-            return B2F_BAD_ARG;
-        }
+        default: return B2F_BAD_ARG;
     }
     return B2F_OK;
 }

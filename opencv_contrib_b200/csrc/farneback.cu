@@ -1152,7 +1152,6 @@ class FarnebackEngine : public b2f_handle {
 public:
     explicit FarnebackEngine(const b2f_farneback_params &p) : P(p) { algo = ALGO_FARNEBACK; }
     b2f_farneback_params P;
-    int num_sms_ = 0;
 
     int calc(const b2f_image *I0, const b2f_image *I1, b2f_image *flow, cudaStream_t s) override;
     int set_param(int id, double v) override;
@@ -1187,16 +1186,16 @@ private:
     Layout L_;
 
     // the whole fixed schedule between the conversion of the caller's frames and the final merge, as one CUDA graph
-    GraphCache graph_;
     struct GraphKey {
-        int rows = 0, cols = 0;
-        b2f_farneback_params P{};
+        int rows, cols;
+        b2f_farneback_params P;
         EngineKnobs knobs;
-        void *base = nullptr;
-    } graph_key_;
-    // b2f_farneback_path of the iteration kernel per solved level: of the last calc (B2F_ENGINE_ACTIVE_PATH) and of
-    // the captured graph
-    std::vector<int> level_paths_, graph_level_paths_;
+        const void *base;
+        bool operator==(const GraphKey &o) const {
+            return rows == o.rows && cols == o.cols && same_params(P, o.P) && same_knobs(knobs, o.knobs) && base == o.base;
+        }
+    };
+    GraphCache<GraphKey> graph_;
     void solve(Ctx &c);
 
     size_t layout(int rows, int cols, bool counting, Layout &L, std::vector<float> &tabs);
@@ -1324,34 +1323,25 @@ int FarnebackEngine::calc(const b2f_image *I0, const b2f_image *I1, b2f_image *f
     Ctx c = make_ctx(s);
     c.check(ensure_workspace(rows, cols, s));
     if (!c.ok()) return finish(c, s);
-    {
-        static bool attr_done[64] = {};
-        int dev = 0;
-        cudaGetDevice(&dev);
-        if (!num_sms_) {
-            cudaDeviceGetAttribute(&num_sms_, cudaDevAttrMultiProcessorCount, dev);
-            if (num_sms_ <= 0) num_sms_ = 132;
-        }
-        if (dev >= 0 && dev < 64 && !attr_done[dev]) {
-            const int bytes = (int)(sizeof(float) * 5 * FT_H * (FT_W + 12));
-            c.check(cudaFuncSetAttribute(k_farn_iter_fast<6, true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes));
-            c.check(cudaFuncSetAttribute(k_farn_iter_fast<6, false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes));
-            c.check(cudaFuncSetAttribute(k_farn_iter_fast<6, true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes));
-            c.check(cudaFuncSetAttribute(k_farn_iter_fast<6, false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes));
-            c.check(cudaFuncSetAttribute(k_farn_iter_fast<6, false, true, 512>, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes));
-            c.check(cudaFuncSetAttribute(k_farn_iter_fast<6, false, true, 256, 3>, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes));
-            c.check(cudaFuncSetAttribute(k_farn_iter_fast<6, false, true, 256, 4>, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes));
-            c.check(cudaFuncSetAttribute(k_farn_iter_fast<6, false, true, 256, 2, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes + 8 * 1024));
-            c.check(cudaFuncSetAttribute(k_farn_iter_tma<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)FARN_TMA_SMEM));
-            c.check(cudaFuncSetAttribute(k_farn_iter_tma<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)FARN_TMA_SMEM));
-            attr_done[dev] = c.ok();
-        }
-    }
+    static DeviceOnce attrs;
+    attrs.run(c, [&] {
+        const int bytes = (int)(sizeof(float) * 5 * FT_H * (FT_W + 12));
+        c.check(cudaFuncSetAttribute(k_farn_iter_fast<6, true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes));
+        c.check(cudaFuncSetAttribute(k_farn_iter_fast<6, false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes));
+        c.check(cudaFuncSetAttribute(k_farn_iter_fast<6, true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes));
+        c.check(cudaFuncSetAttribute(k_farn_iter_fast<6, false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes));
+        c.check(cudaFuncSetAttribute(k_farn_iter_fast<6, false, true, 512>, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes));
+        c.check(cudaFuncSetAttribute(k_farn_iter_fast<6, false, true, 256, 3>, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes));
+        c.check(cudaFuncSetAttribute(k_farn_iter_fast<6, false, true, 256, 4>, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes));
+        c.check(cudaFuncSetAttribute(k_farn_iter_fast<6, false, true, 256, 2, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes + 8 * 1024));
+        c.check(cudaFuncSetAttribute(k_farn_iter_tma<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)FARN_TMA_SMEM));
+        c.check(cudaFuncSetAttribute(k_farn_iter_tma<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)FARN_TMA_SMEM));
+    });
     Layout &L = L_;
     const int top = static_cast<int>(L.levels.size()) - 1;
     stats.levels = top + 1;
     stats.iterations_run = 0;
-    level_paths_.assign(top + 1, 0);
+    active_paths.assign(top + 1, 0.0);
 
     const ImageView v0{I0->data, I0->step, rows, cols, I0->type};
     const ImageView v1{I1->data, I1->step, rows, cols, I1->type};
@@ -1365,22 +1355,7 @@ int FarnebackEngine::calc(const b2f_image *I0, const b2f_image *I1, b2f_image *f
     // replayed: one graph launch instead of ~90 kernel launches per pair (the coarse levels are launch-bound).
     const bool want_graph = knobs.use_graph && !profiling && s != nullptr;
     if (want_graph) {
-        const bool hit = graph_.exec && graph_key_.rows == rows && graph_key_.cols == cols &&
-                         same_params(graph_key_.P, P) && same_knobs(graph_key_.knobs, knobs) &&
-                         graph_key_.base == L.frames[0].p;
-        if (!hit) {
-            graph_.capture(*this, c, [&](Ctx &g) { solve(g); });
-            if (c.ok()) {
-                graph_key_.rows = rows;
-                graph_key_.cols = cols;
-                graph_key_.P = P;
-                graph_key_.knobs = knobs;
-                graph_key_.base = L.frames[0].p;
-                graph_level_paths_ = level_paths_;
-            }
-        }
-        graph_.replay(*this, c, s);
-        if (c.ok()) level_paths_ = graph_level_paths_;
+        graph_.run(*this, c, s, GraphKey{rows, cols, P, knobs, L.frames[0].p}, [&](Ctx &g) { solve(g); });
     } else {
         solve(c);
     }
@@ -1480,17 +1455,17 @@ void FarnebackEngine::solve(Ctx &c) {
         const size_t smem_fast = sizeof(float) * 5 * FT_H * (FT_W + 12);
         // Coarse levels leave most SMs idle and are bound by each thread's chain of dependent round trips (three
         // column tasks, two quad tasks): 512 threads per tile halve that chain.  Same arithmetic, same bits.
-        const bool wide_blocks = (int)(gf.x * gf.y) <= num_sms_ && knobs.fused_iters != 256;
+        const bool wide_blocks = (int)(gf.x * gf.y) <= sm_count() && knobs.fused_iters != 256;
         // opt-in persistent TMA kernel (kernel_path 3) on levels with at least two waves of 64x64 tiles
         const int tma_tx = div_up(w, TT), tma_ty = div_up(h, TT);
-        bool use_tma = knobs.kernel_path == 3 && khalf == 6 && tma_tx * tma_ty >= 2 * num_sms_;
+        bool use_tma = knobs.kernel_path == 3 && khalf == 6 && tma_tx * tma_ty >= 2 * sm_count();
         alignas(64) CUtensorMap mapA, mapB;
         if (use_tma) {
             const uint64_t pitch_b = sizeof(float) * (uint64_t)plane_pitch(w);
             use_tma = tma_encode_2d_f32(&mapA, Ma.p, (uint64_t)w, 5ull * h, pitch_b, TB_W, TB_H) &&
                       tma_encode_2d_f32(&mapB, Mb.p, (uint64_t)w, 5ull * h, pitch_b, TB_W, TB_H);
         }
-        {  // the kernel the loop below launches (same branch order), reported through B2F_ENGINE_ACTIVE_PATH + k
+        {  // the kernel the loop below launches (same branch order), reported as active path k
             const bool quad = knobs.kernel_path != 2;
             int path = B2F_FARN_PATH_GENERIC;
             if (use_tma) path = B2F_FARN_PATH_TMA;
@@ -1501,7 +1476,7 @@ void FarnebackEngine::solve(Ctx &c) {
             else if (fast6 && knobs.aux_path == 5) path = B2F_FARN_PATH_QUAD_TRANSPOSED;
             else if (fast6 && knobs.aux_path == 4) path = B2F_FARN_PATH_QUAD_R64;
             else if (fast6) path = B2F_FARN_PATH_QUAD;
-            level_paths_[k] = P.num_iters > 0 ? path : 0;
+            active_paths[k] = P.num_iters > 0 ? path : 0;
         }
         bool a_is_input = true;
         for (int i = 0; i < P.num_iters; ++i) {
@@ -1510,7 +1485,7 @@ void FarnebackEngine::solve(Ctx &c) {
             const double bytes = npx * (20.0 + (upd ? 60.0 : 0.0) + (wflow ? 8.0 : 0.0));
             if (use_tma) {
                 const int ntiles = tma_tx * tma_ty;
-                const dim3 gt(ntiles < num_sms_ ? ntiles : num_sms_);
+                const dim3 gt(ntiles < sm_count() ? ntiles : sm_count());
                 const CUtensorMap &mapIn = a_is_input ? mapA : mapB;
                 if (gauss)
                     B2F_LAUNCH(c, CLS_ITER, bytes, k_farn_iter_tma<true>, gt, dim3(TNT), FARN_TMA_SMEM, mapIn, Mb, R0, R1,
@@ -1587,12 +1562,7 @@ int FarnebackEngine::get_param(int id, double *v) const {
         case B2F_FARN_POLY_N: *v = P.poly_n; break;
         case B2F_FARN_POLY_SIGMA: *v = P.poly_sigma; break;
         case B2F_FARN_FLAGS: *v = P.flags; break;
-        default:
-            if (id >= B2F_ENGINE_ACTIVE_PATH && id - B2F_ENGINE_ACTIVE_PATH < (int)level_paths_.size()) {
-                *v = level_paths_[id - B2F_ENGINE_ACTIVE_PATH];
-                break;
-            }
-            return B2F_BAD_ARG;
+        default: return B2F_BAD_ARG;
     }
     return B2F_OK;
 }

@@ -103,6 +103,20 @@ b2f::Ctx b2f_handle::make_ctx(cudaStream_t s) {
     return c;
 }
 
+int b2f_handle::sm_count() {
+    if (!sm_count_) {
+        int dev = device, n = 0;
+        if ((dev >= 0 || cudaGetDevice(&dev) == cudaSuccess) &&
+            cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) == cudaSuccess && n > 0) {
+            sm_count_ = n;
+        } else {
+            cudaGetLastError();  // a failed query must not surface as the next launch's error
+            sm_count_ = 132;
+        }
+    }
+    return sm_count_;
+}
+
 int b2f_handle::finish(b2f::Ctx &ctx, cudaStream_t s) {
     if (ctx.ok() && s == nullptr) ctx.check(cudaDeviceSynchronize());  // legacy-stream contract
     if (!ctx.ok()) {
@@ -138,7 +152,7 @@ int b2f_set_param(b2f_handle *h, int id, double value) {
         case B2F_ENGINE_USE_GRAPH: h->knobs.use_graph = value != 0; return B2F_OK;
         case B2F_ENGINE_KERNEL_PATH: h->knobs.kernel_path = static_cast<int>(value); return B2F_OK;
         case B2F_ENGINE_AUX_PATH: h->knobs.aux_path = static_cast<int>(value); return B2F_OK;
-        default: return h->set_param(id, value);
+        default: return id >= B2F_ENGINE_ACTIVE_PATH ? B2F_BAD_ARG : h->set_param(id, value);  // active paths: read-only
     }
 }
 
@@ -149,8 +163,13 @@ int b2f_get_param(const b2f_handle *h, int id, double *value) {
         case B2F_ENGINE_USE_GRAPH: *value = h->knobs.use_graph; return B2F_OK;
         case B2F_ENGINE_KERNEL_PATH: *value = h->knobs.kernel_path; return B2F_OK;
         case B2F_ENGINE_AUX_PATH: *value = h->knobs.aux_path; return B2F_OK;
-        default: return h->get_param(id, value);
+        default: break;
     }
+    if (id < B2F_ENGINE_ACTIVE_PATH) return h->get_param(id, value);
+    const int i = id - B2F_ENGINE_ACTIVE_PATH - h->active_path_first;  // a level the last calc did not solve: BAD_ARG
+    if (i < 0 || i >= static_cast<int>(h->active_paths.size())) return B2F_BAD_ARG;
+    *value = h->active_paths[i];
+    return B2F_OK;
 }
 
 const char *b2f_default_name(const b2f_handle *h) { return h ? h->default_name() : ""; }

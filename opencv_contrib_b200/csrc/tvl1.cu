@@ -530,7 +530,6 @@ public:
         if (iters_host_) cudaFreeHost(iters_host_);
         free(tma_maps_);
         free(warp_maps_);
-        destroy_graph();
     }
 
     b2f_tvl1_params P;
@@ -574,29 +573,24 @@ private:
     void *tma_maps_ = nullptr;
     bool tma_ok_ = false;
     CUtensorMap *warp_maps_ = nullptr;  // one I1 descriptor per level for the tiled warp kernel; null = not available
-    int num_sms_ = 0;
     const void *tma_maps(int level, int cur) const {
         return static_cast<const char *>(tma_maps_) + (size_t)(level * 2 + cur) * tvl1_tma_maps_bytes();
     }
     void blocked_planes(int s, Tvl1BlockedPlanes &B) const;
 
-    // graph cache (fixed schedule only)
-    cudaGraphExec_t graph_exec_ = nullptr;
+    // graph cache (fixed schedule, or epsilon > 0 on the device loop)
     struct GraphKey {
-        int rows = 0, cols = 0, type = -1;
-        b2f_tvl1_params P{};
+        int rows, cols;
+        b2f_tvl1_params P;
         EngineKnobs knobs;
-        int median_filtering = 1, median_period = 0;
-        void *base = nullptr;
-    } graph_key_;
-    uint64_t graph_launches_ = 0;
-    uint64_t graph_class_launches_[B2F_MAX_KERNEL_CLASSES] = {};
-    double graph_class_bytes_[B2F_MAX_KERNEL_CLASSES] = {};
-    int graph_iterations_ = 0;
-    void destroy_graph() {
-        if (graph_exec_) cudaGraphExecDestroy(graph_exec_);
-        graph_exec_ = nullptr;
-    }
+        int median_filtering, median_period;
+        const void *base;
+        bool operator==(const GraphKey &o) const {
+            return rows == o.rows && cols == o.cols && same_params(P, o.P) && same_knobs(knobs, o.knobs) &&
+                   median_filtering == o.median_filtering && median_period == o.median_period && base == o.base;
+        }
+    };
+    GraphCache<GraphKey> graph_;
 
     size_t layout(int rows, int cols, bool counting, Layout &L);
     cudaError_t ensure_workspace(int rows, int cols);
@@ -612,8 +606,8 @@ private:
                          double scaledEps, dim3 grid, dim3 block, int nblocks, int rows, int cols);
     unsigned long long *iters_host_ = nullptr;  // pinned: EpsState::iters_total of the last device-loop solve
     bool device_loop_used_ = false;
-    // b2f_tvl1_path flags per solved level: of the last calc (B2F_ENGINE_ACTIVE_PATH) and of the captured graph
-    std::vector<int> level_paths_, graph_level_paths_;
+    // active paths: an OR of b2f_tvl1_path flags per solved level
+    void mark_path(int s, int flag) { active_paths[s] = static_cast<int>(active_paths[s]) | flag; }
 public:
     void refresh_stats() override {
         if (device_loop_used_ && iters_host_) stats.iterations_run = static_cast<int>(*iters_host_);
@@ -682,7 +676,7 @@ cudaError_t Tvl1Engine::ensure_workspace(int rows, int cols) {
     if (same) return cudaSuccess;
     Layout tmp;
     const size_t need = layout(rows, cols, true, tmp);
-    destroy_graph();
+    graph_.destroy();
     cudaError_t e = arena.reserve(need);
     if (e != cudaSuccess) return e;
     layout(rows, cols, false, L_);
@@ -693,12 +687,6 @@ cudaError_t Tvl1Engine::ensure_workspace(int rows, int cols) {
     if (!err_host) e = cudaMallocHost(&err_host, sizeof(double) * 4);
     if (e != cudaSuccess) return e;
     // TMA descriptors for every solved level and both ping-pong directions
-    if (!num_sms_) {
-        int dev = 0;
-        cudaGetDevice(&dev);
-        cudaDeviceGetAttribute(&num_sms_, cudaDevAttrMultiProcessorCount, dev);
-        if (num_sms_ <= 0) num_sms_ = 132;
-    }
     free(tma_maps_);
     tma_maps_ = nullptr;
     tma_ok_ = false;
@@ -775,9 +763,9 @@ void Tvl1Engine::device_eps_loop(Ctx &c, int s, const Tvl1Planes &T, const Tvl1B
         Ctx b = c;
         b.stream = bs;
         const double npx = (double)rows * cols;
-        level_paths_[s] |= B2F_TVL1_PATH_ITER_TMA | B2F_TVL1_PATH_ITER_UNFUSED;
-        tvl1_tma_launch_dev(b, CLS_ITER, tma_maps(s, 0), B, 0, rows, cols, k, &L_.eps->ia, num_sms_);
-        tvl1_tma_launch_dev(b, CLS_ITER, tma_maps(s, 1), B, 1, rows, cols, k, &L_.eps->ib, num_sms_);
+        mark_path(s, B2F_TVL1_PATH_ITER_TMA | B2F_TVL1_PATH_ITER_UNFUSED);
+        tvl1_tma_launch_dev(b, CLS_ITER, tma_maps(s, 0), B, 0, rows, cols, k, &L_.eps->ia, sm_count());
+        tvl1_tma_launch_dev(b, CLS_ITER, tma_maps(s, 1), B, 1, rows, cols, k, &L_.eps->ib, sm_count());
         B2F_LAUNCH(b, CLS_ITER, 48.0 * npx, k_tvl1_estimate_u, grid, block, 0, T, rows, cols, k, 1, L_.partials,
                    &L_.eps->sample);
         B2F_LAUNCH(b, CLS_REDUCE, 8.0 * nblocks, k_reduce_partials, dim3(1), dim3(256), 0, L_.partials, nblocks,
@@ -848,11 +836,11 @@ void Tvl1Engine::proc_one_scale(Ctx &c, int s, Plane &u3cur, bool allow_sync) {
     };
     auto run_blocked = [&](int count) {
         int done = 0;
-        if (count > 0) level_paths_[s] |= use_tma ? B2F_TVL1_PATH_ITER_TMA : B2F_TVL1_PATH_ITER_BLOCKED;
+        if (count > 0) mark_path(s, use_tma ? B2F_TVL1_PATH_ITER_TMA : B2F_TVL1_PATH_ITER_BLOCKED);
         while (done < count) {
             const int kk = tvl1_blocked_pick_k(knobs.fused_iters, count - done, rows, cols);
             if (use_tma)  // the persistent TMA kernel
-                tvl1_tma_launch(c, CLS_ITER, tma_maps(s, cur), B, cur, rows, cols, k, kk, num_sms_);
+                tvl1_tma_launch(c, CLS_ITER, tma_maps(s, cur), B, cur, rows, cols, k, kk, sm_count());
             else
                 tvl1_blocked_launch(c, CLS_ITER, B, cur, rows, cols, k, kk);
             cur ^= 1;
@@ -881,7 +869,7 @@ void Tvl1Engine::proc_one_scale(Ctx &c, int s, Plane &u3cur, bool allow_sync) {
         // aux_path 3: the separable kernel on every level (40 registers, 6 blocks / SM; the default before the tiled
         // kernel); any other value: the tiled kernel, levels smaller than one staged box the separable one
         const bool tiled = knobs.aux_path != 3 && warp_maps_ && cols >= WB_W && rows >= WB_H;
-        level_paths_[s] |= tiled ? B2F_TVL1_PATH_WARP_TILED : B2F_TVL1_PATH_WARP_UNTILED;
+        mark_path(s, tiled ? B2F_TVL1_PATH_WARP_TILED : B2F_TVL1_PATH_WARP_UNTILED);
         if (tiled)  // I1 window staged by the copy engine
             B2F_LAUNCH(c, CLS_WARP, 32.0 * npx, k_tvl1_warp_tile<4>, dim3(div_up(cols, WT_W), div_up(rows, WT_H)),
                        dim3(WT_THREADS), 0, warp_maps_[s], lv.I0, lv.I1, T.u1, T.u2, T.I1wx, T.I1wy, T.grad, T.rho_c, rows,
@@ -931,7 +919,7 @@ void Tvl1Engine::proc_one_scale(Ctx &c, int s, Plane &u3cur, bool allow_sync) {
                 continue;
             }
             point_T_at(cur);
-            level_paths_[s] |= B2F_TVL1_PATH_ITER_UNFUSED;
+            mark_path(s, B2F_TVL1_PATH_ITER_UNFUSED);
             B2F_LAUNCH(c, CLS_ITER, 48.0 * npx, k_tvl1_estimate_u, grid, block, 0, T, rows, cols, k,
                        calcError ? 1 : 0, L_.partials, nullptr);
             if (calcError) {
@@ -1004,12 +992,12 @@ int Tvl1Engine::calc(const b2f_image *I0, const b2f_image *I1, b2f_image *flow, 
 
     const int rows = I0->rows, cols = I0->cols;
     Ctx c = make_ctx(s);
-    c.check(tvl1_blocked_init());
+    tvl1_blocked_init(c);
     c.check(ensure_workspace(rows, cols));
     if (!c.ok()) return finish(c, s);
     stats.levels = L_.nscales;
     stats.iterations_run = 0;
-    level_paths_.assign(L_.nscales, 0);
+    active_paths.assign(L_.nscales, 0.0);
 
     const ImageView v0{I0->data, I0->step, rows, cols, I0->type};
     const ImageView v1{I1->data, I1->step, rows, cols, I1->type};
@@ -1036,65 +1024,14 @@ int Tvl1Engine::calc(const b2f_image *I0, const b2f_image *I1, b2f_image *flow, 
     const bool want_graph = knobs.use_graph && (fixed_schedule || dev_loop) && !profiling && s != nullptr;
     device_loop_used_ = false;
     if (want_graph) {
-        const bool hit = graph_exec_ && graph_key_.rows == rows && graph_key_.cols == cols &&
-                         same_params(graph_key_.P, P) &&
-                         same_knobs(graph_key_.knobs, knobs) && graph_key_.median_filtering == median_filtering &&
-                         graph_key_.median_period == median_period &&
-                         graph_key_.base == L_.levels[0].I0.p;
-        if (!hit) {
-            destroy_graph();
-            cudaStream_t cs = nullptr;
-            c.check(cudaStreamCreateWithFlags(&cs, cudaStreamNonBlocking));
-            if (c.ok()) {
-                Ctx g = make_ctx(cs);
-                b2f_stats scratch = stats;  // capture must not double-count launches
-                g.stats = &scratch;
-                g.capturing = true;
-                g.check(cudaStreamBeginCapture(cs, cudaStreamCaptureModeThreadLocal));
-                if (g.ok()) solve(g, false);
-                cudaGraph_t graph = nullptr;
-                cudaError_t e = cudaStreamEndCapture(cs, &graph);
-                g.check(e);
-                if (g.ok() && graph) g.check(cudaGraphInstantiate(&graph_exec_, graph, 0));
-                if (graph) cudaGraphDestroy(graph);
-                cudaStreamDestroy(cs);
-                graph_launches_ = scratch.launches - stats.launches;
-                for (int i = 0; i < B2F_MAX_KERNEL_CLASSES; ++i) {
-                    graph_class_launches_[i] = scratch.class_launches[i] - stats.class_launches[i];
-                    graph_class_bytes_[i] = scratch.class_bytes[i] - stats.class_bytes[i];
-                }
-                graph_iterations_ = scratch.iterations_run;
-                graph_level_paths_ = level_paths_;
-                c.check(g.err);
-                if (c.ok()) {
-                    graph_key_.rows = rows;
-                    graph_key_.cols = cols;
-                    graph_key_.P = P;
-                    graph_key_.knobs = knobs;
-                    graph_key_.median_filtering = median_filtering;
-                    graph_key_.median_period = median_period;
-                    graph_key_.base = L_.levels[0].I0.p;
-                } else {
-                    destroy_graph();
-                }
-            }
-        }
-        if (c.ok() && graph_exec_) {
-            c.check(cudaGraphLaunch(graph_exec_, s));
-            stats.launches += graph_launches_;
-            for (int i = 0; i < B2F_MAX_KERNEL_CLASSES; ++i) {
-                stats.class_launches[i] += graph_class_launches_[i];
-                stats.class_bytes[i] += graph_class_bytes_[i];
-            }
-            stats.iterations_run = graph_iterations_;
-            level_paths_ = graph_level_paths_;
-            if (dev_loop) {  // the true count lives on the device: fetch it behind the solve, read it in refresh_stats()
-                if (!iters_host_) c.check(cudaMallocHost(&iters_host_, sizeof(unsigned long long)));
-                if (c.ok())
-                    c.check(cudaMemcpyAsync(iters_host_, &L_.eps->iters_total, sizeof(unsigned long long),
-                                            cudaMemcpyDeviceToHost, s));
-                device_loop_used_ = c.ok();
-            }
+        const GraphKey key{rows, cols, P, knobs, median_filtering, median_period, L_.levels[0].I0.p};
+        if (graph_.run(*this, c, s, key, [&](Ctx &g) { solve(g, false); }) && dev_loop) {
+            // the true count lives on the device: fetch it behind the solve, read it in refresh_stats()
+            if (!iters_host_) c.check(cudaMallocHost(&iters_host_, sizeof(unsigned long long)));
+            if (c.ok())
+                c.check(cudaMemcpyAsync(iters_host_, &L_.eps->iters_total, sizeof(unsigned long long),
+                                        cudaMemcpyDeviceToHost, s));
+            device_loop_used_ = c.ok();
         }
     } else {
         solve(c, true);
@@ -1151,12 +1088,7 @@ int Tvl1Engine::get_param(int id, double *v) const {
         case B2F_TVL1_MEDIAN_FILTERING: *v = median_filtering; break;
         case B2F_TVL1_MEDIAN_PERIOD: *v = median_period; break;
         case B2F_TVL1_INITIAL_FLOW_SOURCE: *v = initial_flow_source; break;
-        default:
-            if (id >= B2F_ENGINE_ACTIVE_PATH && id - B2F_ENGINE_ACTIVE_PATH < (int)level_paths_.size()) {
-                *v = level_paths_[id - B2F_ENGINE_ACTIVE_PATH];
-                break;
-            }
-            return B2F_BAD_ARG;
+        default: return B2F_BAD_ARG;
     }
     return B2F_OK;
 }

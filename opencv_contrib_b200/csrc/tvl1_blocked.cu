@@ -441,16 +441,14 @@ typedef CUresult (*EncodeTiledFn)(CUtensorMap *, CUtensorMapDataType, cuuint32_t
                                   CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
 
 static EncodeTiledFn get_encoder() {
-    static EncodeTiledFn fn = nullptr;
-    static bool tried = false;
-    if (!tried) {
-        tried = true;
+    static const EncodeTiledFn fn = [] {  // a function-local static is initialised once, thread-safely
         void *p = nullptr;
         cudaDriverEntryPointQueryResult q;
-        if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &p, cudaEnableDefault, &q) == cudaSuccess &&
-            q == cudaDriverEntryPointSuccess)
-            fn = reinterpret_cast<EncodeTiledFn>(p);
-    }
+        return cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &p, cudaEnableDefault, &q) == cudaSuccess &&
+                       q == cudaDriverEntryPointSuccess
+                   ? reinterpret_cast<EncodeTiledFn>(p)
+                   : nullptr;
+    }();
     return fn;
 }
 
@@ -581,21 +579,15 @@ void tvl1_tma_launch_dev(Ctx &c, int cls, const void *maps, const Tvl1BlockedPla
                so.p12, so.p21, so.p22, rows, cols, k, 0, halo, tile, tiles_x, ntiles, iters_dev, *out_maps(maps), 1);
 }
 
-cudaError_t tvl1_blocked_init() {
-    static bool done[64] = {};
-    int dev = 0;
-    cudaError_t e = cudaGetDevice(&dev);
-    if (e != cudaSuccess) return e;
-    if (dev >= 0 && dev < 64 && done[dev]) return cudaSuccess;
-    e = cudaFuncSetAttribute(k_tvl1_blocked, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SMEM_BYTES);
-    if (e == cudaSuccess)
-        e = cudaFuncSetAttribute(k_tvl1_blocked_tma<false>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                 (int)smem_tma_bytes());
-    if (e == cudaSuccess)
-        e = cudaFuncSetAttribute(k_tvl1_blocked_tma<true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                 (int)smem_tma_bytes());
-    if (e == cudaSuccess && dev >= 0 && dev < 64) done[dev] = true;
-    return e;
+void tvl1_blocked_init(Ctx &c) {
+    static DeviceOnce attrs;
+    attrs.run(c, [&] {
+        c.check(cudaFuncSetAttribute(k_tvl1_blocked, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SMEM_BYTES));
+        c.check(cudaFuncSetAttribute(k_tvl1_blocked_tma<false>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                     (int)smem_tma_bytes()));
+        c.check(cudaFuncSetAttribute(k_tvl1_blocked_tma<true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                     (int)smem_tma_bytes()));
+    });
 }
 
 int tvl1_blocked_pick_k(int knob, int remaining, int rows, int cols) {

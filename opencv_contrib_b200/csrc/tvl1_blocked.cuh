@@ -35,8 +35,8 @@ struct Tvl1BlockedPlanes {
 
 enum { TVL1_REGION = 64, TVL1_KMAX = 12, TVL1_BLOCK_THREADS = 512 };
 
-// Opt the kernels into >48 KB dynamic shared memory on the current device (idempotent).
-cudaError_t tvl1_blocked_init();
+// Opt the kernels into >48 KB dynamic shared memory on the current device (once per device).
+void tvl1_blocked_init(Ctx &c);
 // K fused iterations for the next launch.
 int tvl1_blocked_pick_k(int knob, int remaining, int rows, int cols);
 // One HBM pass: `iters` iterations from state s[cur] into s[cur^1].

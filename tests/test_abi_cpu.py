@@ -70,19 +70,21 @@ def test_python_mirror_getters_setters_and_names(lib):
 
 def test_null_and_bad_arguments_fail_loudly(lib):
     from opencv_contrib_b200 import _lib
-    h = C.c_void_p()
-    assert lib.b2f_tvl1_create(None, C.byref(h)) == 0 and h.value
     img = _lib.b2f_image(None, 0, 0, 0, 0)
-    assert lib.b2f_calc(h, None, None, None, None) == 1           # B2F_BAD_ARG
-    assert lib.b2f_calc(h, C.byref(img), C.byref(img), C.byref(img), None) == 1
-    assert lib.b2f_set_param(h, 12345, 1.0) == 1
-    v = C.c_double(-1.0)
     active = _lib.PARAM["engine"]["active_path"]
-    assert lib.b2f_get_param(h, active, C.byref(v)) == 1 and v.value == -1.0  # no calc yet: no level to report
-    assert lib.b2f_set_param(h, active, 1.0) == 1                               # read-only
+    for family in ("tvl1", "farneback", "brox", "denselk", "deepflow", "dis"):
+        create = getattr(lib, "b2f_%s_create" % family)
+        h = C.c_void_p()
+        assert create(None, C.byref(h)) == 0 and h.value, family
+        assert lib.b2f_calc(h, None, None, None, None) == 1, family           # B2F_BAD_ARG
+        assert lib.b2f_calc(h, C.byref(img), C.byref(img), C.byref(img), None) == 1, family
+        assert lib.b2f_set_param(h, 12345, 1.0) == 1, family
+        v = C.c_double(-1.0)
+        assert lib.b2f_get_param(h, active, C.byref(v)) == 1 and v.value == -1.0, family  # no calc yet: no level
+        assert lib.b2f_set_param(h, active, 1.0) == 1, family                               # read-only
+        lib.b2f_destroy(h)
+        assert create(None, None) == 1, family
     assert b"B2F_BAD_ARG" in lib.b2f_status_string(1)
-    lib.b2f_destroy(h)
-    assert lib.b2f_tvl1_create(None, None) == 1
 
 
 def test_active_path_ids_match_header():
