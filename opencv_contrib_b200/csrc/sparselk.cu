@@ -40,6 +40,8 @@ namespace b2f {
 namespace {
 
 constexpr int SB = 256;  // 16 x 16 threads per point (pyrlk.cpp:116-133 calcPatchSize, compute >= 1.2)
+constexpr int RED = 3 * (SB / 32);  // block_sum's staging (`red`): the kernels' only static shared memory
+constexpr size_t STATIC_SMEM = RED * sizeof(float);
 
 struct TexView {
     Plane p;
@@ -92,7 +94,7 @@ __global__ void __launch_bounds__(SB) k_sparse_lk(TexView I, TexView J, const fl
     extern __shared__ float sp_smem[];
     const int n_win = win_x * win_y;
     float *I_patch = sp_smem, *dIdx_patch = sp_smem + n_win, *dIdy_patch = sp_smem + 2 * n_win;
-    __shared__ float red[24];
+    __shared__ float red[RED];
     const int tid = threadIdx.x;
     const int pt = blockIdx.x;
     const int rows = I.rows, cols = I.cols;
@@ -233,7 +235,7 @@ __global__ void __launch_bounds__(SB) k_sparse_lk_mc(TexViewN I, TexViewN J, con
     extern __shared__ float sp_smem[];
     const int n_win = win_x * win_y;
     float *I_patch = sp_smem, *dIdx_patch = sp_smem + CN * n_win, *dIdy_patch = sp_smem + 2 * CN * n_win;
-    __shared__ float red[24];
+    __shared__ float red[RED];
     const int tid = threadIdx.x;
     const int pt = blockIdx.x;
     const int rows = I.rows, cols = I.cols;
@@ -360,6 +362,31 @@ __global__ void k_sparse_init(const float2 *__restrict__ src, float2 *__restrict
     status[i] = 1;                                    // status.setTo(1), :173-174
 }
 
+// cudaDevAttrMaxSharedMemoryPerBlockOptin of the current device, queried once per device; 0 when the query fails
+int smem_optin_limit() {
+    constexpr int kMaxDevices = 64;
+    static std::atomic<int> cache[kMaxDevices] = {};
+    int dev = -1;
+    if (cudaGetDevice(&dev) != cudaSuccess) {
+        cudaGetLastError();
+        return 0;
+    }
+    const bool tracked = dev >= 0 && dev < kMaxDevices;
+    if (tracked) {
+        const int v = cache[dev].load(std::memory_order_relaxed);
+        if (v > 0) return v;
+    }
+    int v = 0;
+    if (cudaDeviceGetAttribute(&v, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev) != cudaSuccess) {
+        cudaGetLastError();
+        return 0;
+    }
+    if (tracked) cache[dev].store(v, std::memory_order_relaxed);
+    return v;
+}
+
+bool aligned(const void *p, size_t a) { return reinterpret_cast<uintptr_t>(p) % a == 0; }
+
 }  // namespace
 }  // namespace b2f
 
@@ -417,6 +444,7 @@ int b2f_sparselk_calc(b2f_sparse *h, const b2f_image *prev_img, const b2f_image 
     if (next_img->type != prev_img->type) return B2F_UNSUPPORTED_TYPE;                                 // pyrlk.cpp:229
     if (prev_img->rows != next_img->rows || prev_img->cols != next_img->cols) return B2F_SIZE_MISMATCH;
     if (P.max_level < 0 || !(P.win_width > 2 && P.win_height > 2) || P.iters < 0) return B2F_BAD_ARG;  // :160-161
+    if (P.max_level > 30) return B2F_BAD_ARG;  // 1 << (max_level + 1) and the kernels' 1 << level must stay defined
     // calcPatchSize + CV_Assert(patch.x < 6 && patch.y < 6), pyrlk.cpp:116-133,184
     const bool wide = P.win_width > 32 && P.win_width > 2 * P.win_height;
     const int bx = wide ? 32 : 16, by = wide ? 8 : 16;
@@ -424,10 +452,21 @@ int b2f_sparselk_calc(b2f_sparse *h, const b2f_image *prev_img, const b2f_image 
     const size_t es = (depth == 0 ? 1 : depth == 2 ? 2 : 4) * (size_t)cn;
     if (prev_img->step < prev_img->cols * es || next_img->step < next_img->cols * es) return B2F_BAD_ARG;
     if (depth != 0 && ((prev_img->step | next_img->step) % (es / cn)) != 0) return B2F_BAD_ARG;
+    if (!aligned(prev_img->data, es / cn) || !aligned(next_img->data, es / cn)) return B2F_BAD_ARG;  // element reads
+    if (!aligned(prev_pts, sizeof(float2)) || !aligned(next_pts, sizeof(float2)) || !aligned(err, sizeof(float)))
+        return B2F_BAD_ARG;  // the kernels read and write points as float2
     const int rows = prev_img->rows, cols = prev_img->cols;
     cudaStream_t s = static_cast<cudaStream_t>(cuda_stream);
     DeviceScope dev(prev_img->data, s);
     const bool legacy = cn == 1 && (depth == 0 || depth == 5);  // single-plane texture-path kernel
+    // Each point's block keeps its I, dI/dx and dI/dy patches in shared memory, 12 * cn bytes per window element.  The
+    // reference holds them in registers and accepts every window calcPatchSize allows (up to 80 x 80 or 160 x 40); here
+    // a patch that does not fit next to the static staging in the device's opt-in shared memory per block is refused.
+    const size_t smem = sizeof(float) * 3 * (size_t)cn * P.win_width * P.win_height;
+    const int optin_max = smem_optin_limit();
+    if (optin_max <= 0) return B2F_CUDA_ERROR;
+    if (smem + STATIC_SMEM > (size_t)optin_max) return B2F_BAD_ARG;
+    const bool optin = smem + STATIC_SMEM > 48 * 1024;  // the default limit counts static and dynamic memory together
 
     Ctx c;
     c.stream = s;
@@ -460,11 +499,10 @@ int b2f_sparselk_calc(b2f_sparse *h, const b2f_image *prev_img, const b2f_image 
         }
     }
     const int half_x = (P.win_width - 1) / 2, half_y = (P.win_height - 1) / 2;
-    const size_t smem = sizeof(float) * 3 * (size_t)cn * P.win_width * P.win_height;
     const float scale = static_cast<float>(1.0 / (1 << P.max_level) / 2.0);
     const float2 *init_src = reinterpret_cast<const float2 *>(P.use_initial_flow ? next_pts : prev_pts);
     if (c.ok() && legacy) {
-        if (smem > 48 * 1024)
+        if (optin)
             c.check(cudaFuncSetAttribute(k_sparse_lk, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
         const ImageView v0{prev_img->data, prev_img->step, rows, cols, prev_img->type};
         const ImageView v1{next_img->data, next_img->step, rows, cols, next_img->type};
@@ -537,7 +575,7 @@ int b2f_sparselk_calc(b2f_sparse *h, const b2f_image *prev_img, const b2f_image 
         B2F_LAUNCH(c, 2, 17.0 * n_points, k_sparse_init, dim3(div_up(n_points, 256)), dim3(256), 0, init_src,
                    reinterpret_cast<float2 *>(next_pts), status, n_points, scale);
         auto launch = [&](auto kernel) {
-            if (smem > 48 * 1024) c.check(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+            if (optin) c.check(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
             for (int l = P.max_level; l >= 0; --l) {
                 TexViewN tI = view(h->I, l), tJ = view(h->J, l);
                 B2F_LAUNCH(c, 0, 0.0, kernel, dim3(n_points), dim3(SB), smem, tI, tJ, reinterpret_cast<const float2 *>(prev_pts),
