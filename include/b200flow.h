@@ -165,6 +165,26 @@ typedef struct b2f_dis_params {
 /* cv::DISOpticalFlow::PRESET_* */
 enum { B2F_DIS_PRESET_ULTRAFAST = 0, B2F_DIS_PRESET_FAST = 1, B2F_DIS_PRESET_MEDIUM = 2 };
 
+/* cv::cuda::FastOpticalFlowBM (modules/cudalegacy/include/opencv2/cudalegacy.hpp:202-211; src/bm_fast.cpp:62-88,
+ * src/cuda/bm_fast.cu).  Dense integer block matching: for every pixel the offset (x, y) in
+ * [-sr, search_window - 1 - sr]^2, sr = search_window / 2, whose block_window x block_window sum of absolute differences
+ * between I0 and I1 is least; both frames are extended with cudev's reflect-101 rule (one fold and a modulo, not the
+ * CPU's iterative borderInterpolate).  Ties go to the least (k mod 128, k div 128) for k = y * search_window + x, as the
+ * reference's 128-thread scan and reduction decide them.  Inputs 8UC1 of equal size (anything else:
+ * B2F_UNSUPPORTED_TYPE), output 32FC2 (b2f_calc) or two 32FC1 planes (b2f_calc_uv, how the reference returns it); the
+ * caller's flow is never read, so the video front end runs it without warm start.  Refused with B2F_BAD_ARG:
+ *   search_window outside 1..109: the reference's kernel needs 4 * search_window^2 bytes of dynamic plus 1024 bytes of
+ *       static shared memory without opting in to more than 48 KB, so 109 is its largest working size;
+ *   an even block_window: the reference's column ring then overruns into the next CTA's buffer rows (a race);
+ *   block_window above 31: this engine's warp keeps 32 - (block_window - 1) output columns (the reference has no limit).
+ * The reference class is not a cv::Algorithm; b2f_default_name reports "DenseOpticalFlow.FastOpticalFlowBM".
+ * B2F_ENGINE_ACTIVE_PATH + 0 after a calc: bits 0-7 the output columns per warp, bits 8-15 the tile rows, bit 16 set
+ * when the (SAD, rank) key was compared in 64 bits (the window pair could overflow 32). */
+typedef struct b2f_fastbm_params {
+    int search_window; /* 21 */
+    int block_window;  /* 7  */
+} b2f_fastbm_params;
+
 typedef struct b2f_handle b2f_handle;
 
 /* ---- construction: replaces the static ::create() factories.  A NULL params pointer means
@@ -177,6 +197,7 @@ B2F_API void b2f_brox_default_params(b2f_brox_params *p);
 B2F_API void b2f_denselk_default_params(b2f_denselk_params *p);
 B2F_API void b2f_deepflow_default_params(b2f_deepflow_params *p);
 B2F_API void b2f_dis_default_params(b2f_dis_params *p, int preset); /* DISOpticalFlow::create(preset) */
+B2F_API void b2f_fastbm_default_params(b2f_fastbm_params *p);
 
 B2F_API int b2f_tvl1_create(const b2f_tvl1_params *p, b2f_handle **out);           /* src/tvl1flow.cpp:385-391 */
 B2F_API int b2f_farneback_create(const b2f_farneback_params *p, b2f_handle **out); /* src/farneback.cpp:484-489 */
@@ -184,6 +205,7 @@ B2F_API int b2f_brox_create(const b2f_brox_params *p, b2f_handle **out);        
 B2F_API int b2f_denselk_create(const b2f_denselk_params *p, b2f_handle **out);     /* src/pyrlk.cpp:402-405 */
 B2F_API int b2f_deepflow_create(const b2f_deepflow_params *p, b2f_handle **out);   /* optflow deepflow.cpp:171-174 */
 B2F_API int b2f_dis_create(const b2f_dis_params *p, b2f_handle **out);             /* NULL: the FAST preset */
+B2F_API int b2f_fastbm_create(const b2f_fastbm_params *p, b2f_handle **out);       /* cudalegacy.hpp:202-211 */
 B2F_API void b2f_destroy(b2f_handle *h);
 
 /* ---- getters/setters: replace getTau()/setTau() ... (cudaoptflow.hpp:158-177,233-243,261-283,
@@ -221,6 +243,8 @@ typedef enum b2f_param_id {
     B2F_DIS_GRADIENT_DESCENT_ITERATIONS, B2F_DIS_VARIATIONAL_REFINEMENT_ITERATIONS, B2F_DIS_VARIATIONAL_REFINEMENT_ALPHA,
     B2F_DIS_VARIATIONAL_REFINEMENT_DELTA, B2F_DIS_VARIATIONAL_REFINEMENT_GAMMA, B2F_DIS_VARIATIONAL_REFINEMENT_EPSILON,
     B2F_DIS_USE_MEAN_NORMALIZATION, B2F_DIS_USE_SPATIAL_PROPAGATION, B2F_DIS_USE_INITIAL_FLOW,
+    /* FastOpticalFlowBM */
+    B2F_FBM_SEARCH_WINDOW = 700, B2F_FBM_BLOCK_WINDOW,
     /* engine knobs (no reference counterpart) */
     B2F_ENGINE_FUSED_ITERS = 900, /* TV-L1: inner iterations fused per HBM pass (0 = auto)     */
     B2F_ENGINE_USE_GRAPH = 901,   /* capture the fixed schedule in a CUDA graph (default 1)    */
@@ -382,9 +406,31 @@ B2F_API int b2f_interpolate_frames(const b2f_image *frame0, const b2f_image *fra
                                    const b2f_image *fv, const b2f_image *bu, const b2f_image *bv, float pos,
                                    b2f_image *new_frame, b2f_image *buf, int flags, void *cuda_stream);
 
+/* ---- cv::cuda::calcOpticalFlowBM (cudalegacy.hpp:196-200; src/bm.cpp:60-202, src/cuda/bm.cu:56-160): one vector
+ *      per grid cell.  velSize = ((cols - bw + sw) / sw, (rows - bh + sh) / sh) for block (bw, bh) and shift (sw, sh);
+ *      cell (i, j) compares the block at (j sw, i sh) of `curr` with `prev` at the candidate offsets (the reference's
+ *      cmpBlocks receives its frames swapped: if curr is prev shifted by +s, the result is -s, kept for drop-in
+ *      parity).  Candidates follow the reference's spiral over [-max_range, max_range]^2 minus the origin, relative to the
+ *      start offset (the rounded previous velocity with use_previous, else 0); a candidate whose SAD is below
+ *      2 bw bh is taken at once, ties with the best SAD are averaged, and a best above 128 bw bh falls back to the
+ *      start offset.  The spiral is computed on the device, so no table buffer is needed.
+ *   prev, curr : device 8UC1 of one size (else B2F_UNSUPPORTED_TYPE / B2F_SIZE_MISMATCH).
+ *   velx, vely : device 32FC1 of velSize (else B2F_SIZE_MISMATCH), read first when use_previous is set.
+ *   B2F_BAD_ARG: a block or shift side below 1, a range below 0 or above B2F_BM_MAX_RANGE, 128 bw bh above INT_MAX (the
+ *      reference's escape level overflows), or an empty velSize.
+ *   Asynchronous on `stream` like b2f_calc (a NULL stream ends with a device synchronise). ---- */
+enum { B2F_BM_MAX_RANGE = 16383 };
+B2F_API int b2f_calc_optical_flow_bm_size(int rows, int cols, int block_width, int block_height, int shift_width,
+                                          int shift_height, int max_range_width, int max_range_height, int *vel_rows,
+                                          int *vel_cols, int *table_len);
+B2F_API int b2f_calc_optical_flow_bm(const b2f_image *prev, const b2f_image *curr, int block_width, int block_height,
+                                     int shift_width, int shift_height, int max_range_width, int max_range_height,
+                                     int use_previous, b2f_image *velx, b2f_image *vely, void *cuda_stream);
+
 /* ---- batched frame-pair front end for one GPU (SURVEY.md 8b / 8e): N engine handles on N streams, pairs dealt
  *      round robin -- the pattern of the reference's own multi-stream test (test/test_optflow.cpp:468-528).
- *      algo: 1 TV-L1, 2 Farneback, 3 Brox, 4 DensePyrLK, 5 DeepFlow, 6 DIS; params: the matching b2f_*_params (NULL = defaults).
+ *      algo: 1 TV-L1, 2 Farneback, 3 Brox, 4 DensePyrLK, 5 DeepFlow, 6 DIS, 7 FastOpticalFlowBM; params: the matching
+ *      b2f_*_params (NULL = defaults).
  *      Sharding over GPUs / processes and the NCCL result gather stay with the caller's process framework
  *      (opencv_contrib_b200/batch.py over torch.distributed). ---- */
 typedef struct b2f_batch b2f_batch;

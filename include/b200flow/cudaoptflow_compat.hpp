@@ -325,6 +325,60 @@ public:
     }
 };
 
+/** cv::cuda::FastOpticalFlowBM (cudalegacy.hpp:202-211): operator() with the reference's signature; flowx / flowy are
+ *  (re)allocated as CV_32FC1 of the frame's size.  Also a DenseOpticalFlow (calc writes CV_32FC2 with the handle's
+ *  windows).  Refused windows: see b2f_fastbm_params. */
+class FastOpticalFlowBM : public DenseOpticalFlow, protected impl::HandleOwner {
+public:
+    FastOpticalFlowBM() {
+        const int st = b2f_fastbm_create(nullptr, &h_);
+        if (st != B2F_OK) detail::fail(st, "FastOpticalFlowBM");
+    }
+    B2F_ACCESSOR(int, SearchWindow, B2F_FBM_SEARCH_WINDOW)
+    B2F_ACCESSOR(int, BlockWindow, B2F_FBM_BLOCK_WINDOW)
+
+    void operator()(const GpuMat &I0, const GpuMat &I1, GpuMat &flowx, GpuMat &flowy, int search_window = 21,
+                    int block_window = 7, Stream &stream = Stream::Null()) {
+        setSearchWindow(search_window);
+        setBlockWindow(block_window);
+        flowx.create(I0.rows, I0.cols, 5 /*CV_32FC1*/);
+        flowy.create(I0.rows, I0.cols, 5 /*CV_32FC1*/);
+        b2f_image i0{I0.data, I0.step, I0.rows, I0.cols, I0.type()};
+        b2f_image i1{I1.data, I1.step, I1.rows, I1.cols, I1.type()};
+        b2f_image u{flowx.data, flowx.step, flowx.rows, flowx.cols, flowx.type()};
+        b2f_image v{flowy.data, flowy.step, flowy.rows, flowy.cols, flowy.type()};
+        const int st = b2f_calc_uv(h_, &i0, &i1, &u, &v, detail::raw(stream));
+        if (st != B2F_OK) detail::fail(st, "FastOpticalFlowBM::operator()");
+    }
+    void calc(InputArray I0, InputArray I1, InputOutputArray flow, Stream &stream = Stream::Null()) override {
+        run(I0, I1, flow, stream, false);
+    }
+    String getDefaultName() const override { return b2f_default_name(h_); }
+};
+
+/** cv::cuda::calcOpticalFlowBM (cudalegacy.hpp:196-200), the reference's signature.  velx / vely are (re)allocated as
+ *  CV_32FC1 of velSize unless use_previous is set, when they are read first and must already be of velSize.  `buf` is
+ *  accepted and left untouched: the spiral table is computed on the device. */
+inline void calcOpticalFlowBM(const GpuMat &prev, const GpuMat &curr, Size block_size, Size shift_size, Size max_range,
+                              bool use_previous, GpuMat &velx, GpuMat &vely, GpuMat &buf, Stream &stream = Stream::Null()) {
+    (void)buf;
+    int vr = 0, vc = 0;
+    int st = b2f_calc_optical_flow_bm_size(prev.rows, prev.cols, block_size.width, block_size.height, shift_size.width,
+                                           shift_size.height, max_range.width, max_range.height, &vr, &vc, nullptr);
+    if (st != B2F_OK) detail::fail(st, "calcOpticalFlowBM");
+    if (!use_previous) {
+        velx.create(vr, vc, 5 /*CV_32FC1*/);
+        vely.create(vr, vc, 5 /*CV_32FC1*/);
+    }
+    b2f_image p{prev.data, prev.step, prev.rows, prev.cols, prev.type()};
+    b2f_image c{curr.data, curr.step, curr.rows, curr.cols, curr.type()};
+    b2f_image x{velx.data, velx.step, velx.rows, velx.cols, velx.type()};
+    b2f_image y{vely.data, vely.step, vely.rows, vely.cols, vely.type()};
+    st = b2f_calc_optical_flow_bm(&p, &c, block_size.width, block_size.height, shift_size.width, shift_size.height,
+                                  max_range.width, max_range.height, use_previous ? 1 : 0, &x, &y, detail::raw(stream));
+    if (st != B2F_OK) detail::fail(st, "calcOpticalFlowBM");
+}
+
 #undef B2F_ACCESSOR
 
 /** cv::cuda::SparsePyrLKOpticalFlow (cudaoptflow.hpp:189-226), same signature as the reference's

@@ -28,6 +28,8 @@ from .cudaoptflow import (  # noqa: F401
     DISOPTICAL_FLOW_PRESET_ULTRAFAST,
     DISOPTICAL_FLOW_PRESET_FAST,
     DISOPTICAL_FLOW_PRESET_MEDIUM,
+    FastOpticalFlowBM,
+    calcOpticalFlowBM,
     SparsePyrLKOpticalFlow,
     SparsePyrLKOpticalFlow_create,
     OPTFLOW_USE_INITIAL_FLOW,

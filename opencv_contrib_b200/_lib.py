@@ -63,6 +63,10 @@ class b2f_dis_params(C.Structure):
                 ("use_spatial_propagation", C.c_int), ("use_initial_flow", C.c_int)]
 
 
+class b2f_fastbm_params(C.Structure):
+    _fields_ = [("search_window", C.c_int), ("block_window", C.c_int)]
+
+
 class b2f_sparselk_params(C.Structure):
     _fields_ = [("win_width", C.c_int), ("win_height", C.c_int), ("max_level", C.c_int), ("iters", C.c_int),
                 ("use_initial_flow", C.c_int)]
@@ -99,6 +103,10 @@ SYMBOLS = [
     ("b2f_denselk_create", C.c_int, [C.POINTER(b2f_denselk_params), C.POINTER(_H)]),
     ("b2f_deepflow_create", C.c_int, [C.POINTER(b2f_deepflow_params), C.POINTER(_H)]),
     ("b2f_dis_create", C.c_int, [C.POINTER(b2f_dis_params), C.POINTER(_H)]),
+    ("b2f_fastbm_default_params", None, [C.POINTER(b2f_fastbm_params)]),
+    ("b2f_fastbm_create", C.c_int, [C.POINTER(b2f_fastbm_params), C.POINTER(_H)]),
+    ("b2f_calc_optical_flow_bm_size", C.c_int, [C.c_int] * 8 + [C.POINTER(C.c_int)] * 3),
+    ("b2f_calc_optical_flow_bm", C.c_int, [_IMG, _IMG] + [C.c_int] * 7 + [_IMG, _IMG, C.c_void_p]),
     ("b2f_destroy", None, [_H]),
     ("b2f_set_param", C.c_int, [_H, C.c_int, C.c_double]),
     ("b2f_get_param", C.c_int, [_H, C.c_int, C.POINTER(C.c_double)]),
@@ -173,6 +181,7 @@ PARAM = {
     "dis": dict(finest_scale=600, coarsest_scale=601, patch_size=602, patch_stride=603, grad_descent_iterations=604,
                 variational_refinement_iterations=605, alpha=606, delta=607, gamma=608, epsilon=609,
                 use_mean_normalization=610, use_spatial_propagation=611, use_initial_flow=612),
+    "fastbm": dict(search_window=700, block_window=701),
     "engine": dict(fused_iters=900, use_graph=901, kernel_path=902, aux_path=903, active_path=1000),
 }
 # b2f_tvl1_path flags (include/b200flow.h)

@@ -104,8 +104,8 @@ int b2f_video_create(b2f_handle *h, int rows, int cols, int type, int depth, int
             v->warm_param = B2F_DIS_USE_INITIAL_FLOW;
             v->warm_on = 1;
             v->warm_off = 0;
-        } else {  // Brox, DensePyrLK and DeepFlow have no initial-flow path (brox.cpp:129-188, pyrlk.cpp:238-299,
-                  // deepflow.cpp:132,146)
+        } else {  // Brox, DensePyrLK, DeepFlow and FastBM have no initial-flow path (brox.cpp:129-188, pyrlk.cpp:238-299,
+                  // deepflow.cpp:132,146, cudalegacy bm_fast.cpp:62-88)
             delete v;
             return B2F_BAD_ARG;
         }

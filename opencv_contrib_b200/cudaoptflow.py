@@ -366,6 +366,66 @@ def DISOpticalFlow_create(preset=DISOPTICAL_FLOW_PRESET_FAST):
     return _create(DISOpticalFlow, "b2f_dis_create", p)
 
 
+class FastOpticalFlowBM(DenseOpticalFlow):
+    """cv::cuda::FastOpticalFlowBM (cudalegacy.hpp:202-211): dense integer block matching on u8 frames.
+
+        flowx, flowy = FastOpticalFlowBM()(I0, I1[, flowx[, flowy[, search_window[, block_window[, stream]]]]])
+
+    as in the reference, plus the inherited calc / calcUV with the handle's own windows (setSearchWindow /
+    setBlockWindow).  The caller's flow is never read.  Refused windows: see b2f_fastbm_params."""
+
+    def __init__(self, handle=None, search_window=21, block_window=7):
+        if handle is None:
+            p = _lib.b2f_fastbm_params(search_window, block_window)
+            handle = C.c_void_p()
+            st = _lib.lib().b2f_fastbm_create(C.byref(p), C.byref(handle))
+            if st != 0:
+                raise B2FError(st)
+        super().__init__(handle)
+
+    def __call__(self, I0, I1, flowx=None, flowy=None, search_window=21, block_window=7, stream=None):
+        self.setSearchWindow(search_window)
+        self.setBlockWindow(block_window)
+        return self.calcUV(I0, I1, flowx, flowy, stream)
+
+    def getActivePath(self):
+        """(output columns per warp, tile rows, 64-bit key) of the last calc (B2F_ENGINE_ACTIVE_PATH)."""
+        v = int(self._get(PARAM["engine"]["active_path"]))
+        return v & 0xFF, (v >> 8) & 0xFF, bool((v >> 16) & 1)
+
+
+_accessors(FastOpticalFlowBM, "fastbm", {"search_window": ("SearchWindow", int), "block_window": ("BlockWindow", int)})
+
+
+def calcOpticalFlowBM(prev, curr, block_size, shift_size, max_range, use_previous, velx=None, vely=None, stream=None):
+    """cv::cuda::calcOpticalFlowBM (cudalegacy.hpp:196-200) -> (velx, vely), float32 of velSize.  block_size,
+    shift_size and max_range are (width, height), as cv::Size.  With use_previous, velx / vely are read first (and
+    must be given); otherwise they are allocated when missing.  The reference's `buf` argument is not needed: the
+    spiral table is computed on the device."""
+    torch = _torch()
+    l = _lib.lib()
+    vr, vc, n = C.c_int(), C.c_int(), C.c_int()
+    st = l.b2f_calc_optical_flow_bm_size(prev.shape[0], prev.shape[1], block_size[0], block_size[1], shift_size[0],
+                                         shift_size[1], max_range[0], max_range[1], C.byref(vr), C.byref(vc), C.byref(n))
+    if st != 0:
+        raise B2FError(st)
+    if velx is None or vely is None:
+        if use_previous:
+            raise B2FError(3)
+        velx = torch.empty((vr.value, vc.value), dtype=torch.float32, device=prev.device)
+        vely = torch.empty_like(velx)
+    i0, i1, ix, iy = (_image_from_tensor(t) for t in (prev, curr, velx, vely))
+    if stream is None:
+        stream = torch.cuda.current_stream(prev.device)
+    sptr = stream.cuda_stream if hasattr(stream, "cuda_stream") else int(stream)
+    st = l.b2f_calc_optical_flow_bm(C.byref(i0), C.byref(i1), block_size[0], block_size[1], shift_size[0],
+                                    shift_size[1], max_range[0], max_range[1], int(bool(use_previous)), C.byref(ix),
+                                    C.byref(iy), C.c_void_p(sptr))
+    if st != 0:
+        raise B2FError(st)
+    return velx, vely
+
+
 def _sparse_image(t) -> b2f_image:
     """(H, W) or (H, W, C) CUDA tensor, C in {1, 3, 4}, dtype uint8 / uint16 / int32 / float32 -> b2f_image with OpenCV's
     CV_MAKETYPE(depth, C) flag: the instantiations of the reference's sparse dispatcher table (pyrlk.cpp:195-203)."""

@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """Twin of the reference's evaluation sample (modules/optflow/samples/optical_flow_evaluation.cpp):
 
-    python tools/flow_eval.py image1 image2 {tvl1,farneback,brox,denselk,dis_ultrafast,dis_fast,dis_medium}
+    python tools/flow_eval.py image1 image2 {tvl1,farneback,brox,denselk,dis_ultrafast,dis_fast,dis_medium,fastbm}
                               [groundtruth.flo]
                               [-m endpoint|angular|angular-fixed] [-o out.flo]
 
@@ -20,7 +20,7 @@ def main():
     ap.add_argument("image1")
     ap.add_argument("image2")
     ap.add_argument("algorithm", choices=["tvl1", "farneback", "brox", "denselk", "dis_ultrafast", "dis_fast",
-                                                  "dis_medium"])
+                                                  "dis_medium", "fastbm"])
     ap.add_argument("groundtruth", nargs="?")
     ap.add_argument("-m", "--measure", default="endpoint", choices=["endpoint", "angular", "angular-fixed"])
     ap.add_argument("-o", "--out")
@@ -44,7 +44,7 @@ def main():
         d1, d2 = torch.from_numpy(i1).to(dev), torch.from_numpy(i2).to(dev)
     else:
         alg = {"tvl1": ocb.OpticalFlowDual_TVL1_create, "farneback": ocb.FarnebackOpticalFlow_create,
-               "denselk": ocb.DensePyrLKOpticalFlow_create}[a.algorithm]()
+               "denselk": ocb.DensePyrLKOpticalFlow_create, "fastbm": ocb.FastOpticalFlowBM}[a.algorithm]()
         d1, d2 = torch.from_numpy(i1).to(dev), torch.from_numpy(i2).to(dev)
     flow = alg.calc(d1, d2, torch.zeros((*i1.shape, 2), dtype=torch.float32, device=dev))
     torch.cuda.synchronize()
