@@ -554,6 +554,64 @@ B2F_API int b2f_flow_error_stats(const float *err, size_t err_step, const unsign
 B2F_API int b2f_flow_accuracy(const float *gold, size_t gold_step, const float *flow, size_t flow_step, int rows,
                               int cols, double threshold, double *fraction);
 
+/* ---- superres: cv::superres::createSuperResolution_BTVL1_CUDA (modules/superres/src/btv_l1_cuda.cpp, src/cuda/
+ *      btv_l1_gpu.cu): bilateral total-variation L1 multi-frame super-resolution of a video, on the optical flows of one of
+ *      the engines above (TV-L1, Farneback, Brox or DensePyrLK through b2f_calc_ext's conversion) or of flows the caller
+ *      supplies.  Frames are device 8UC1, 8UC3 or 8UC4 (anything else: B2F_UNSUPPORTED_TYPE) of one size per stream
+ *      (else B2F_SIZE_MISMATCH).  The reference's pull schedule (nextFrame reads 2R + 1 frames first, then one per output)
+ *      runs in the library: while b2f_superres_wants_frame says so, push the next frame (NULL = end of stream); then
+ *      b2f_superres_pop returns the next output, rows*scale - 2 btv_kernel_size by cols*scale - 2 btv_kernel_size, as
+ *      8UC{1,3,4} (the reference's nextFrame) or 32FC{1,3,4} (the float estimate before convertTo), until it reports no
+ *      output at the end.  N frames give N outputs.  scale and temporal_area_radius are read when a stream's first frame
+ *      arrives; the other parameters each time a frame is processed.  Every reference CV_Assert (btv_l1_cuda.cpp:310-316)
+ *      plus an even or > 31 blur size, a radius above B2F_SR_MAX_RADIUS or an output of no pixels returns B2F_BAD_ARG
+ *      from the push or pop that would process.  All work is on `cuda_stream`, without host synchronisation
+ *      (a NULL stream ends each call with a device synchronise). ---- */
+typedef struct b2f_superres_params {
+    int scale;                /* 4    */
+    int iterations;           /* 180  */
+    double tau;               /* 1.3  */
+    double lambda;            /* 0.03 */
+    double alpha;             /* 0.7  */
+    int btv_kernel_size;      /* 7    */
+    int blur_kernel_size;     /* 5    */
+    double blur_sigma;        /* 0.0  */
+    int temporal_area_radius; /* 4    */
+} b2f_superres_params;
+enum { B2F_SR_MAX_RADIUS = 15 };
+enum {
+    B2F_SR_SCALE = 800, B2F_SR_ITERATIONS, B2F_SR_TAU, B2F_SR_LAMBDA, B2F_SR_ALPHA, B2F_SR_BTV_KERNEL_SIZE,
+    B2F_SR_BLUR_KERNEL_SIZE, B2F_SR_BLUR_SIGMA, B2F_SR_TEMPORAL_AREA_RADIUS
+};
+typedef struct b2f_superres b2f_superres;
+B2F_API void b2f_superres_default_params(b2f_superres_params *p);
+/* flow: a TV-L1, Farneback, Brox or DensePyrLK handle (borrowed, else B2F_BAD_ARG), or NULL: the caller pushes flows */
+B2F_API int b2f_superres_create(const b2f_superres_params *p, b2f_handle *flow, b2f_superres **out);
+B2F_API int b2f_superres_set_flow(b2f_superres *sr, b2f_handle *flow);
+B2F_API int b2f_superres_set_param(b2f_superres *sr, int id, double value); /* also B2F_ENGINE_USE_GRAPH */
+B2F_API int b2f_superres_get_param(const b2f_superres *sr, int id, double *value);
+B2F_API int b2f_superres_wants_frame(const b2f_superres *sr, int *wants);
+/* readNextFrame: with a flow engine; frame NULL = end of stream */
+B2F_API int b2f_superres_push(b2f_superres *sr, const b2f_image *frame, void *cuda_stream);
+/* without one: the frame with 32FC1 flows previous -> frame (fwd) and frame -> previous (bwd); ignored for the first */
+B2F_API int b2f_superres_push_flows(b2f_superres *sr, const b2f_image *frame, const b2f_image *fwd_u,
+                                    const b2f_image *fwd_v, const b2f_image *bwd_u, const b2f_image *bwd_v,
+                                    void *cuda_stream);
+/* *produced = 1 when `out` received the next output, 0 at the end of the stream */
+B2F_API int b2f_superres_pop(b2f_superres *sr, b2f_image *out, int *produced, void *cuda_stream);
+B2F_API int b2f_superres_output_size(const b2f_superres *sr, int *rows, int *cols); /* after the first frame */
+B2F_API int b2f_superres_reset(b2f_superres *sr);           /* a new stream */
+B2F_API int b2f_superres_collect_garbage(b2f_superres *sr); /* a new stream, device memory released */
+B2F_API int b2f_superres_get_stats(b2f_superres *sr, b2f_stats *out);
+B2F_API int b2f_superres_reset_stats(b2f_superres *sr);
+B2F_API int b2f_superres_last_cuda_error(const b2f_superres *sr);
+B2F_API void b2f_superres_destroy(b2f_superres *sr);
+/* superres's GpuOpticalFlow::calc (superres/src/optical_flow.cpp:456-497): 8UC{1,3,4} frames of one type and size are
+ * converted to the engine's work type (cudev's 15-bit BGR(A)->gray rule, then x float(1/255) for Brox's 32FC1, 8UC1 for
+ * the others), then flow1 = interleaved 32FC2, or with flow2 planar u / v 32FC1.  TV-L1, Farneback, Brox, DensePyrLK. */
+B2F_API int b2f_calc_ext(b2f_handle *h, const b2f_image *I0, const b2f_image *I1, b2f_image *flow1, b2f_image *flow2,
+                         void *cuda_stream);
+
 #ifdef __cplusplus
 }
 #endif

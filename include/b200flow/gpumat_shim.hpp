@@ -13,7 +13,7 @@ namespace b200flow {
 namespace shim {
 
 enum { CV_8U = 0, CV_32F = 5 };
-enum { CV_8UC1 = 0, CV_32FC1 = 5, CV_32FC2 = 13 };
+enum { CV_8UC1 = 0, CV_32FC1 = 5, CV_32FC2 = 13, CV_8UC3 = 16, CV_32FC3 = 21, CV_8UC4 = 24, CV_32FC4 = 29 };
 
 struct Size {
     int width = 0, height = 0;
@@ -56,10 +56,14 @@ public:
 
     GpuMat() = default;
     GpuMat(int r, int c, int t) { create(r, c, t); }
-    static size_t elemSize(int t) { return t == CV_8UC1 ? 1 : t == CV_32FC1 ? 4 : t == CV_32FC2 ? 8 : 0; }
+    // 8U or 32F with 1 to 4 channels (OpenCV's CV_MAKETYPE layout: depth in bits 0-2, channels - 1 above)
+    static size_t elemSize(int t) {
+        const int d = t & 7;
+        return d == CV_8U ? (size_t)((t >> 3) + 1) : d == CV_32F ? (size_t)4 * ((t >> 3) + 1) : 0;
+    }
     int type() const { return flags; }
-    int channels() const { return flags == CV_32FC2 ? 2 : 1; }
-    int depth() const { return flags == CV_8UC1 ? CV_8U : CV_32F; }
+    int channels() const { return (flags >> 3) + 1; }
+    int depth() const { return flags & 7; }
     size_t elemSize() const { return elemSize(flags); }
     Size size() const { return Size(cols, rows); }
     bool empty() const { return data == nullptr; }

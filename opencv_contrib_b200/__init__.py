@@ -10,6 +10,7 @@ Only what the hot path needs lives here:
   video.py         consecutive-frame front end (one upload per frame, warm start, 3-stream pipeline)
   frames.py        interpolateFrames, the consumer right after the solvers
   flowio.py        Middlebury .flo files + the reference's error statistics
+  superres.py      superres's BTV-L1 video super-resolution and its four CUDA optical-flow wrappers
 """
 from .cudaoptflow import (  # noqa: F401
     DenseOpticalFlow,
@@ -39,3 +40,10 @@ from ._lib import B2FError  # noqa: F401
 from .frames import interpolateFrames  # noqa: F401
 from .video import VideoFlow  # noqa: F401
 from . import flowio  # noqa: F401
+from .superres import (  # noqa: F401
+    createSuperResolution_BTVL1_CUDA,
+    createOptFlow_Farneback_CUDA,
+    createOptFlow_DualTVL1_CUDA,
+    createOptFlow_Brox_CUDA,
+    createOptFlow_PyrLK_CUDA,
+)

@@ -72,6 +72,12 @@ class b2f_sparselk_params(C.Structure):
                 ("use_initial_flow", C.c_int)]
 
 
+class b2f_superres_params(C.Structure):
+    _fields_ = [("scale", C.c_int), ("iterations", C.c_int), ("tau", C.c_double), ("lambda_", C.c_double),
+                ("alpha", C.c_double), ("btv_kernel_size", C.c_int), ("blur_kernel_size", C.c_int),
+                ("blur_sigma", C.c_double), ("temporal_area_radius", C.c_int)]
+
+
 class b2f_stats(C.Structure):
     _fields_ = [("calls", C.c_uint64), ("launches", C.c_uint64),
                 ("class_launches", C.c_uint64 * B2F_MAX_KERNEL_CLASSES),
@@ -155,6 +161,23 @@ SYMBOLS = [
     ("b2f_batch_launches", C.c_uint64, [_H]),
     ("b2f_batch_reset_stats", C.c_int, [_H]),
     ("b2f_batch_destroy", None, [_H]),
+    ("b2f_superres_default_params", None, [C.POINTER(b2f_superres_params)]),
+    ("b2f_superres_create", C.c_int, [C.POINTER(b2f_superres_params), _H, C.POINTER(_H)]),
+    ("b2f_superres_set_flow", C.c_int, [_H, _H]),
+    ("b2f_superres_set_param", C.c_int, [_H, C.c_int, C.c_double]),
+    ("b2f_superres_get_param", C.c_int, [_H, C.c_int, C.POINTER(C.c_double)]),
+    ("b2f_superres_wants_frame", C.c_int, [_H, C.POINTER(C.c_int)]),
+    ("b2f_superres_push", C.c_int, [_H, _IMG, C.c_void_p]),
+    ("b2f_superres_push_flows", C.c_int, [_H, _IMG, _IMG, _IMG, _IMG, _IMG, C.c_void_p]),
+    ("b2f_superres_pop", C.c_int, [_H, _IMG, C.POINTER(C.c_int), C.c_void_p]),
+    ("b2f_superres_output_size", C.c_int, [_H, C.POINTER(C.c_int), C.POINTER(C.c_int)]),
+    ("b2f_superres_reset", C.c_int, [_H]),
+    ("b2f_superres_collect_garbage", C.c_int, [_H]),
+    ("b2f_superres_get_stats", C.c_int, [_H, C.POINTER(b2f_stats)]),
+    ("b2f_superres_reset_stats", C.c_int, [_H]),
+    ("b2f_superres_last_cuda_error", C.c_int, [_H]),
+    ("b2f_superres_destroy", None, [_H]),
+    ("b2f_calc_ext", C.c_int, [_H, _IMG, _IMG, _IMG, _IMG, C.c_void_p]),
     ("b2f_flo_read_size", C.c_int, [C.c_char_p, C.POINTER(C.c_int), C.POINTER(C.c_int)]),
     ("b2f_flo_read", C.c_int, [C.c_char_p, C.c_void_p, C.c_size_t, C.c_int, C.c_int]),
     ("b2f_flo_write", C.c_int, [C.c_char_p, C.c_void_p, C.c_size_t, C.c_int, C.c_int]),
@@ -182,6 +205,8 @@ PARAM = {
                 variational_refinement_iterations=605, alpha=606, delta=607, gamma=608, epsilon=609,
                 use_mean_normalization=610, use_spatial_propagation=611, use_initial_flow=612),
     "fastbm": dict(search_window=700, block_window=701),
+    "superres": dict(scale=800, iterations=801, tau=802, lambda_=803, alpha=804, btv_kernel_size=805,
+                     blur_kernel_size=806, blur_sigma=807, temporal_area_radius=808),
     "engine": dict(fused_iters=900, use_graph=901, kernel_path=902, aux_path=903, active_path=1000),
 }
 # b2f_tvl1_path flags (include/b200flow.h)

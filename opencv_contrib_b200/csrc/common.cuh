@@ -210,6 +210,9 @@ struct b2f_handle {
     // staging for b2f_calc_host
     void *host_stage = nullptr;
     size_t host_stage_bytes = 0;
+    // work-type frames of b2f_calc_ext
+    void *ext_stage = nullptr;
+    size_t ext_stage_bytes = 0;
 
     virtual ~b2f_handle();
     virtual int calc(const b2f_image *I0, const b2f_image *I1, b2f_image *flow, cudaStream_t s) = 0;

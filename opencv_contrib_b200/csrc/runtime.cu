@@ -91,6 +91,7 @@ b2f_handle::~b2f_handle() {
     }
     for (auto e : event_pool) cudaEventDestroy(e);
     if (host_stage) cudaFree(host_stage);
+    if (ext_stage) cudaFree(ext_stage);
 }
 
 b2f::Ctx b2f_handle::make_ctx(cudaStream_t s) {
