@@ -319,6 +319,11 @@ typedef enum b2f_tvl1_path {
  * cv::cuda has no float median filter).  Pitched device planes (step a multiple of 4 bytes). */
 B2F_API int b2f_median_blur_32f(const b2f_image *src, b2f_image *dst, int ksize, void *cuda_stream);
 
+/* Test support: out[i] = op(in[i]) for n device floats, through the very approximations the kernels use
+ * (op 0: rcp.approx.ftz.f32, op 1: sqrt.approx.ftz.f32; one MUFU instruction each on sm_90a), so that a test can
+ * tabulate them and check a model of them on every input.  NULL stream: synchronous. */
+B2F_API int b2f_approx_probe(int op, const float *in, float *out, size_t n, void *cuda_stream);
+
 B2F_API int b2f_set_param(b2f_handle *h, int id, double value);
 B2F_API int b2f_get_param(const b2f_handle *h, int id, double *value);
 

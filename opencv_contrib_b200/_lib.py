@@ -104,6 +104,7 @@ SYMBOLS = [
     ("b2f_dis_default_params", None, [C.POINTER(b2f_dis_params), C.c_int]),
     ("b2f_tvl1_create", C.c_int, [C.POINTER(b2f_tvl1_params), C.POINTER(_H)]),
     ("b2f_median_blur_32f", C.c_int, [C.POINTER(b2f_image), C.POINTER(b2f_image), C.c_int, C.c_void_p]),
+    ("b2f_approx_probe", C.c_int, [C.c_int, C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]),
     ("b2f_farneback_create", C.c_int, [C.POINTER(b2f_farneback_params), C.POINTER(_H)]),
     ("b2f_brox_create", C.c_int, [C.POINTER(b2f_brox_params), C.POINTER(_H)]),
     ("b2f_denselk_create", C.c_int, [C.POINTER(b2f_denselk_params), C.POINTER(_H)]),

@@ -24,7 +24,10 @@ __global__ void k_convert_pair(const T *__restrict__ sa, const T *__restrict__ s
 }
 
 // cv::cuda::resize INTER_LINEAR float C1: src = dst * scale, x2/y2 reads clamped, weights from the
-// unclamped neighbours (cudawarping/src/cuda/resize.cu:234-269).  `mul` fuses the flow rescale.
+// unclamped neighbours (cudawarping/src/cuda/resize.cu:234-269).  `mul` fuses the flow rescale.  The reference's
+// `out = out + src * (w_x * w_y)` is written out as the rounding nvcc contracts it into: each weight product rounded on
+// its own, then one fused multiply-add per tap, the first one onto +0.  The remaining plain expressions here and in
+// k_convert_pair / k_copy_plane are single rounded operations with nothing to contract.
 __device__ __forceinline__ float resize_sample(const Plane &s, int srows, int scols, int dx, int dy, float inv_fx,
                                                float inv_fy) {
     const float src_x = dx * inv_fx;
@@ -37,10 +40,10 @@ __device__ __forceinline__ float resize_sample(const Plane &s, int srows, int sc
     const float wx2 = x2 - src_x, wx1 = src_x - x1;
     const float wy2 = y2 - src_y, wy1 = src_y - y1;
     float out = 0.f;
-    out = out + __ldg(&s.at(y1r, x1r)) * (wx2 * wy2);
-    out = out + __ldg(&s.at(y1r, x2r)) * (wx1 * wy2);
-    out = out + __ldg(&s.at(y2r, x1r)) * (wx2 * wy1);
-    out = out + __ldg(&s.at(y2r, x2r)) * (wx1 * wy1);
+    out = __fmaf_rn(__ldg(&s.at(y1r, x1r)), __fmul_rn(wx2, wy2), out);
+    out = __fmaf_rn(__ldg(&s.at(y1r, x2r)), __fmul_rn(wx1, wy2), out);
+    out = __fmaf_rn(__ldg(&s.at(y2r, x1r)), __fmul_rn(wx2, wy1), out);
+    out = __fmaf_rn(__ldg(&s.at(y2r, x2r)), __fmul_rn(wx1, wy1), out);
     return out;
 }
 

@@ -2,6 +2,7 @@
 // C ABI declared in include/b200flow.h.
 #include "common.cuh"
 
+#include <algorithm>
 #include <cmath>
 #include <cstring>
 #include <new>
@@ -141,8 +142,28 @@ void b2f_handle::collect_profile() {
     timed.clear();
 }
 
+namespace {
+// b2f_approx_probe: rcp_approx / sqrt_approx from common.cuh, the functions the TV-L1 kernels call, element-wise
+__global__ void k_approx_probe(int op, const float *__restrict__ in, float *__restrict__ out, size_t n) {
+    for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x)
+        out[i] = op == 0 ? b2f::rcp_approx(in[i]) : b2f::sqrt_approx(in[i]);
+}
+}  // namespace
+
 // ------------------------------------------------------------------------------------ C ABI (generic part)
 extern "C" {
+
+int b2f_approx_probe(int op, const float *in, float *out, size_t n, void *cuda_stream) {
+    if (!(op == 0 || op == 1) || (n && (!in || !out))) return B2F_BAD_ARG;
+    if (n == 0) return B2F_OK;
+    cudaStream_t s = static_cast<cudaStream_t>(cuda_stream);
+    b2f::DeviceScope dev(in, s);
+    const size_t blocks = std::min<size_t>((n + 255) / 256, 65535 * 8);
+    k_approx_probe<<<(unsigned)blocks, 256, 0, s>>>(op, in, out, n);
+    cudaError_t e = cudaGetLastError();
+    if (e == cudaSuccess && s == nullptr) e = cudaDeviceSynchronize();
+    return e == cudaSuccess ? B2F_OK : B2F_CUDA_ERROR;
+}
 
 void b2f_destroy(b2f_handle *h) { delete h; }
 

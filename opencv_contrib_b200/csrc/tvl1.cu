@@ -57,10 +57,10 @@ __device__ __noinline__ void warp_border_taps(const Plane I1, int rows, int cols
         for (int i = 0; i < 4; ++i) {
             const int cx = clampi(ix + i, 0, cols - 1);
             const int cxp = min(cx + 1, cols - 1), cxm = max(cx - 1, 0);
-            const float w = kx[i] * ky[j];
+            const float w = __fmul_rn(kx[i], ky[j]);
             const float v = __ldg(&I1.at(cy, cx));
-            const float gx = 0.5f * (__ldg(&I1.at(cy, cxp)) - __ldg(&I1.at(cy, cxm)));
-            const float gy = 0.5f * (__ldg(&I1.at(cyp, cx)) - __ldg(&I1.at(cym, cx)));
+            const float gx = __fmul_rn(0.5f, __fsub_rn(__ldg(&I1.at(cy, cxp)), __ldg(&I1.at(cy, cxm))));
+            const float gy = __fmul_rn(0.5f, __fsub_rn(__ldg(&I1.at(cyp, cx)), __ldg(&I1.at(cym, cx))));
             sum = __fmaf_rn(w, v, sum);
             sumx = __fmaf_rn(w, gx, sumx);
             sumy = __fmaf_rn(w, gy, sumy);
@@ -70,7 +70,12 @@ __device__ __noinline__ void warp_border_taps(const Plane I1, int rows, int cols
 
 // Keys a = -0.5 weights of the four taps at distances (1 + t, t, 1 - t, 2 - t), t in [0, 1): the reference's bicubic
 // polynomials (tvl1flow.cu:89-104) expanded in t (same values up to rounding; t itself is exact, the reference rounds
-// t + 1 and 2 - t).
+// t + 1 and 2 - t).  Left as plain expressions on purpose: written with rounding intrinsics, the same operations come out
+// with a different register allocation in the 40-register warp kernels.  nvcc contracts them (cuobjdump -sass) into
+//   k0 = fmul(fma(fma(-0.5, t, 1), t, -0.5), t)       k1 = fma(fmul(fma(1.5, t, -2.5), t), t, 1)
+//   k2 = fmul(fma(fma(-1.5, t, 2), t, 0.5), t)         k3 = fmul(fmul(fma(0.5, t, -0.5), t), t)
+// while the weight sums ((k0 + k1) + (k2 + k3)) of both axes and their product stay single rounded adds and one multiply;
+// oracle/tvl1_gpu_model.c (ENGINE_ROUNDING) restates exactly this.
 __device__ __forceinline__ void keys_weights(float t, float (&k)[4]) {
     k[0] = ((-0.5f * t + 1.0f) * t - 0.5f) * t;
     k[1] = (1.5f * t - 2.5f) * t * t + 1.0f;
@@ -99,15 +104,15 @@ __global__ void __launch_bounds__(256, MINB) k_tvl1_warp_sep(Plane I0, Plane I1,
     const float u1 = __ldg(&u1p.at(y, x));
     const float u2 = __ldg(&u2p.at(y, x));
     const float I0v = __ldg(&I0.at(y, x));
-    const float wx = x + u1;
-    const float wy = y + u2;
+    const float wx = __fadd_rn(static_cast<float>(x), u1);
+    const float wy = __fadd_rn(static_cast<float>(y), u2);
     const float fx = floorf(wx), fy = floorf(wy);
     const int ix = static_cast<int>(fminf(fmaxf(fx, -8.f), cols + 8.f)) - 1;
     const int iy = static_cast<int>(fminf(fmaxf(fy, -8.f), rows + 8.f)) - 1;
 
     float kx[4], ky[4];
-    keys_weights(wx - fx, kx);
-    keys_weights(wy - fy, ky);
+    keys_weights(__fsub_rn(wx, fx), kx);
+    keys_weights(__fsub_rn(wy, fy), ky);
     float sum, sumx, sumy;
     const float wsum = ((kx[0] + kx[1]) + (kx[2] + kx[3])) * ((ky[0] + ky[1]) + (ky[2] + ky[3]));
 
@@ -118,23 +123,28 @@ __global__ void __launch_bounds__(256, MINB) k_tvl1_warp_sep(Plane I0, Plane I1,
         for (int j = 0; j < 6; ++j) {
             const float *row = base + (size_t)j * I1.pitch;
             const float a1 = __ldg(row + 1), a2 = __ldg(row + 2), a3 = __ldg(row + 3), a4 = __ldg(row + 4);
-            r[j] = __fmaf_rn(kx[3], a4, __fmaf_rn(kx[2], a3, __fmaf_rn(kx[1], a2, kx[0] * a1)));
+            r[j] = __fmaf_rn(kx[3], a4, __fmaf_rn(kx[2], a3, __fmaf_rn(kx[1], a2, __fmul_rn(kx[0], a1))));
             if (j >= 1 && j <= 4) {
                 const float a0 = __ldg(row), a5 = __ldg(row + 5);
-                rx[j - 1] = __fmaf_rn(kx[3], a5 - a3, __fmaf_rn(kx[2], a4 - a2, __fmaf_rn(kx[1], a3 - a1, kx[0] * (a2 - a0))));
+                rx[j - 1] = __fmaf_rn(kx[3], __fsub_rn(a5, a3),
+                                      __fmaf_rn(kx[2], __fsub_rn(a4, a2),
+                                                __fmaf_rn(kx[1], __fsub_rn(a3, a1), __fmul_rn(kx[0], __fsub_rn(a2, a0)))));
             }
         }
-        sum = __fmaf_rn(ky[3], r[4], __fmaf_rn(ky[2], r[3], __fmaf_rn(ky[1], r[2], ky[0] * r[1])));
-        sumx = 0.5f * __fmaf_rn(ky[3], rx[3], __fmaf_rn(ky[2], rx[2], __fmaf_rn(ky[1], rx[1], ky[0] * rx[0])));
-        sumy = 0.5f * __fmaf_rn(ky[3], r[5] - r[3], __fmaf_rn(ky[2], r[4] - r[2], __fmaf_rn(ky[1], r[3] - r[1], ky[0] * (r[2] - r[0]))));
+        sum = __fmaf_rn(ky[3], r[4], __fmaf_rn(ky[2], r[3], __fmaf_rn(ky[1], r[2], __fmul_rn(ky[0], r[1]))));
+        sumx = __fmul_rn(0.5f, __fmaf_rn(ky[3], rx[3],
+                         __fmaf_rn(ky[2], rx[2], __fmaf_rn(ky[1], rx[1], __fmul_rn(ky[0], rx[0])))));
+        sumy = __fmul_rn(0.5f, __fmaf_rn(ky[3], __fsub_rn(r[5], r[3]),
+                         __fmaf_rn(ky[2], __fsub_rn(r[4], r[2]),
+                                   __fmaf_rn(ky[1], __fsub_rn(r[3], r[1]), __fmul_rn(ky[0], __fsub_rn(r[2], r[0]))))));
     } else {
         warp_border_taps(I1, rows, cols, ix, iy, kx, ky, sum, sumx, sumy);  // out of line: keeps the hot path's registers low
     }
 
     const float coeff = 1.0f / wsum;
-    const float I1w = sum * coeff;
-    const float Ix = sumx * coeff;
-    const float Iy = sumy * coeff;
+    const float I1w = __fmul_rn(sum, coeff);
+    const float Ix = __fmul_rn(sumx, coeff);
+    const float Iy = __fmul_rn(sumy, coeff);
     I1wx.at(y, x) = Ix;
     I1wy.at(y, x) = Iy;
     grad.at(y, x) = tvl1_inv_grad(__fmaf_rn(Iy, Iy, __fmul_rn(Ix, Ix)));  // the thresholding constant, not |grad|^2
@@ -179,15 +189,20 @@ __device__ __forceinline__ void warp_sep_window(const float *base, size_t pitch,
         const float *row = STRIDE ? base + j * STRIDE : base + (size_t)j * pitch;
         const float a1 = STRIDE ? row[1] : __ldg(row + 1), a2 = STRIDE ? row[2] : __ldg(row + 2);
         const float a3 = STRIDE ? row[3] : __ldg(row + 3), a4 = STRIDE ? row[4] : __ldg(row + 4);
-        r[j] = __fmaf_rn(kx[3], a4, __fmaf_rn(kx[2], a3, __fmaf_rn(kx[1], a2, kx[0] * a1)));
+        r[j] = __fmaf_rn(kx[3], a4, __fmaf_rn(kx[2], a3, __fmaf_rn(kx[1], a2, __fmul_rn(kx[0], a1))));
         if (j >= 1 && j <= 4) {
             const float a0 = STRIDE ? row[0] : __ldg(row), a5 = STRIDE ? row[5] : __ldg(row + 5);
-            rx[j - 1] = __fmaf_rn(kx[3], a5 - a3, __fmaf_rn(kx[2], a4 - a2, __fmaf_rn(kx[1], a3 - a1, kx[0] * (a2 - a0))));
+            rx[j - 1] = __fmaf_rn(kx[3], __fsub_rn(a5, a3),
+                                  __fmaf_rn(kx[2], __fsub_rn(a4, a2),
+                                            __fmaf_rn(kx[1], __fsub_rn(a3, a1), __fmul_rn(kx[0], __fsub_rn(a2, a0)))));
         }
     }
-    sum = __fmaf_rn(ky[3], r[4], __fmaf_rn(ky[2], r[3], __fmaf_rn(ky[1], r[2], ky[0] * r[1])));
-    sumx = 0.5f * __fmaf_rn(ky[3], rx[3], __fmaf_rn(ky[2], rx[2], __fmaf_rn(ky[1], rx[1], ky[0] * rx[0])));
-    sumy = 0.5f * __fmaf_rn(ky[3], r[5] - r[3], __fmaf_rn(ky[2], r[4] - r[2], __fmaf_rn(ky[1], r[3] - r[1], ky[0] * (r[2] - r[0]))));
+    sum = __fmaf_rn(ky[3], r[4], __fmaf_rn(ky[2], r[3], __fmaf_rn(ky[1], r[2], __fmul_rn(ky[0], r[1]))));
+    sumx = __fmul_rn(0.5f, __fmaf_rn(ky[3], rx[3],
+                     __fmaf_rn(ky[2], rx[2], __fmaf_rn(ky[1], rx[1], __fmul_rn(ky[0], rx[0])))));
+    sumy = __fmul_rn(0.5f, __fmaf_rn(ky[3], __fsub_rn(r[5], r[3]),
+                     __fmaf_rn(ky[2], __fsub_rn(r[4], r[2]),
+                               __fmaf_rn(ky[1], __fsub_rn(r[3], r[1]), __fmul_rn(ky[0], __fsub_rn(r[2], r[0]))))));
 }
 
 // Pixels whose window left the staged box (flow beyond the margin) or touches the image border.  A real call on purpose;
@@ -206,21 +221,21 @@ __device__ __noinline__ float3 warp_slow_taps(const Plane I1, int rows, int cols
 // Per-pixel set-up and write-back shared by the two phases of the tiled kernel (same expressions as k_tvl1_warp_sep).
 __device__ __forceinline__ void warp_px_setup(int x, int y, float u1, float u2, int rows, int cols, int &ix, int &iy,
                                               float (&kx)[4], float (&ky)[4], float &wsum) {
-    const float wx = x + u1;
-    const float wy = y + u2;
+    const float wx = __fadd_rn(static_cast<float>(x), u1);
+    const float wy = __fadd_rn(static_cast<float>(y), u2);
     const float fx = floorf(wx), fy = floorf(wy);
     ix = static_cast<int>(fminf(fmaxf(fx, -8.f), cols + 8.f)) - 1;
     iy = static_cast<int>(fminf(fmaxf(fy, -8.f), rows + 8.f)) - 1;
-    keys_weights(wx - fx, kx);
-    keys_weights(wy - fy, ky);
+    keys_weights(__fsub_rn(wx, fx), kx);
+    keys_weights(__fsub_rn(wy, fy), ky);
     wsum = ((kx[0] + kx[1]) + (kx[2] + kx[3])) * ((ky[0] + ky[1]) + (ky[2] + ky[3]));
 }
 __device__ __forceinline__ void warp_px_finish(int x, int y, float u1, float u2, float I0v, float sum, float sumx, float sumy,
                                                float wsum, Plane I1wx, Plane I1wy, Plane grad, Plane rho) {
     const float coeff = 1.0f / wsum;
-    const float I1w = sum * coeff;
-    const float Ix = sumx * coeff;
-    const float Iy = sumy * coeff;
+    const float I1w = __fmul_rn(sum, coeff);
+    const float Ix = __fmul_rn(sumx, coeff);
+    const float Iy = __fmul_rn(sumy, coeff);
     I1wx.at(y, x) = Ix;
     I1wy.at(y, x) = Iy;
     grad.at(y, x) = tvl1_inv_grad(__fmaf_rn(Iy, Iy, __fmul_rn(Ix, Ix)));  // the thresholding constant, not |grad|^2
@@ -348,7 +363,7 @@ __global__ void __launch_bounds__(256) k_tvl1_estimate_u(Tvl1Planes P, int rows,
         P.u1.at(y, x) = u1n;
         P.u2.at(y, x) = u2n;
         if (calc_error) {
-            const float d1 = u1 - u1n, d2 = u2 - u2n;  // u3 is not part of the GPU error (:284-286)
+            const float d1 = __fsub_rn(u1, u1n), d2 = __fsub_rn(u2, u2n);  // u3 is not part of the GPU error (:284-286)
             err = __fmaf_rn(d2, d2, __fmul_rn(d1, d1));
         }
     }

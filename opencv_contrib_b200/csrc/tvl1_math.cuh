@@ -4,7 +4,9 @@
 // contract mul+add pairs.  Semantics follow the reference kernels:
 //   estimateUKernel             modules/cudaoptflow/src/cuda/tvl1flow.cu:209-288
 //   estimateDualVariablesKernel modules/cudaoptflow/src/cuda/tvl1flow.cu:313-348
-// Deliberate arithmetic choices (documented in DESIGN.md, covered by the tolerance tests):
+// Deliberate arithmetic choices (documented in DESIGN.md; oracle/tvl1_gpu_model.c built with -DENGINE_ROUNDING restates
+// each of them, and the engine equals that model bit for bit in tests/test_tvl1_gpu.py and test_tvl1_fullsize_gpu.py,
+// rcp.approx / sqrt.approx emulated from tables of the device's own values):
 //   * -rho/grad is -rho * rcp.approx(grad) (MUFU.RCP, <= 2 ulp) instead of an IEEE divide, and the
 //     three-way threshold test is written as the equivalent clamp (see tvl1_threshold);
 //   * hypotf(a,b) is sqrt.approx(a*a + b*b) and the dual normalisation multiplies by a shared

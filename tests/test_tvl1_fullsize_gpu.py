@@ -5,27 +5,27 @@ residue, the tiled warp kernel's switch to the separable fallback, sub-region im
 Default knobs, CUDA graph on, a real stream.  Every case first asserts which kernels ran (getActivePath), so a
 shape that silently falls back to the plain-load kernels fails instead of passing vacuously.
 
-Tolerances (see DESIGN.md "Parity"):
-  * staged-window fallback (1080p, one level, initial flows up to 40 px): max |dflow| <= 1e-3 px against the float
-    model, the small-size bound;
+The engine is compared with the engine-rounding model ("eng" build, fed this device's rcp.approx / sqrt.approx
+tables) bit for bit, as uint32 views, in every case: the shape sweep, both BASELINE sizes on the TMA and the unfused
+kernels, the staged-window fallback at every initial-flow amplitude, and the reference defaults whenever the engine ran
+as many iterations as the model.  The tolerances that used to bound the engine now bound that model against the float
+model, with the double model as the yardstick (see DESIGN.md "Parity"), so the engine inherits them:
+  * staged-window fallback (1080p, one level, initial flows up to 40 px): max |dflow| <= 1e-3 px;
   * shape sweep (one level, 2 warps x 30 iterations = passes of 8 + 8 + 8 + 6): max |dflow| <= 1e-3 px and the 99 %
-    quantile <= 1e-4 px against the float model, each raised to 4 x the float-vs-double figure where float rounding
-    alone moves the flow further (2513 x 221, seed 22: one ill-conditioned pixel moves 5.1e-3 px between the float
-    and the double model);
-  * BASELINE sizes (5 scales x 10 warps x 30 iterations): at the 50 %, 99 %, 99.9 % quantiles and the max, the
-    end-point error of the engine against the float model is at most 4 x that of the float model against the
-    double model on the same input -- float rounding alone moves the flow that far (at 1080p the max is ~0.02 px,
-    so a fixed 1e-3 bound cannot hold), and rcp.approx / sqrt.approx in the engine add rounding of the same order;
+    quantile <= 1e-4 px, each raised to 4 x the float-vs-double figure where float rounding alone moves the flow
+    further (2513 x 221, seed 22: one ill-conditioned pixel moves 5.1e-3 px between the float and the double model);
+  * BASELINE sizes (5 scales x 10 warps x 30 iterations): at the 50 %, 99 %, 99.9 % quantiles and the max, at most
+    4 x the float model's distance from the double model on the same input (at 1080p the max of that is ~0.02 px);
   * reference defaults at 1080p (epsilon = 0.01, device-side WHILE loop): the iteration count equals the model's
-    per-warp trace summed, unless a sampled error sum lay within 1e-5 (relative) of its threshold; the flow as in
-    the sweep.
+    per-warp trace summed, unless a sampled error sum lay within 1e-5 (relative) of its threshold (the device sums
+    its error image in another order than the model); the flow as in the sweep.
 """
 import time
 
 import numpy as np
 import pytest
 
-from oracle import metrics, synth, tvl1_gpu_model as gm, tvl1_gpu_model_native as nm
+from oracle import metrics, mufu, synth, tvl1_gpu_model as gm, tvl1_gpu_model_native as nm
 
 pytestmark = pytest.mark.gpu
 
@@ -39,19 +39,29 @@ FLOORS = {0.99: 1e-4, 1.0: 1e-3}  # the small-size bounds, for the sweep and the
 
 
 def _check_vs_yardstick(e, yard, floors, label):
-    """Quantiles of e = EPE(engine, float model) against FACTOR x the same quantiles of yard = EPE(float model, double
-    model); floors: {quantile: bound} checked instead wherever it is the larger (None: all QUANTILES, no floor)."""
+    """Quantiles of e = EPE(engine-rounding model, float model) against FACTOR x the same quantiles of
+    yard = EPE(float model, double model); floors: {quantile: bound} checked instead wherever it is the larger (None:
+    all QUANTILES, no floor)."""
     for q in (QUANTILES if floors is None else sorted(floors)):
         v, y = float(np.quantile(e, q)), float(np.quantile(yard, q))
         bound = max(FACTOR * y, 0.0 if floors is None else floors[q])
-        print(f"{label}: q{q:g} engine-vs-f32 {v:.2e}, f32-vs-f64 {y:.2e}, bound {bound:.2e}")
+        print(f"{label}: q{q:g} eng-vs-f32 {v:.2e}, f32-vs-f64 {y:.2e}, bound {bound:.2e}")
         assert v <= bound, (label, q, v, y, _worst_tiles(e))
 
 
+def _assert_bits(got, exact, label):
+    """The engine equals the engine-rounding model bit for bit; on failure, how many values differ and the worst
+    pixels with their position in the 48 x 48 centre tile."""
+    assert got.shape == exact.shape and exact.dtype == np.float32, (label, got.shape, exact.shape)
+    diff = got.view(np.uint32) != exact.view(np.uint32)
+    assert not diff.any(), (label, int(diff.sum()), _worst_tiles(metrics.epe(got, exact)))
+
+
 @pytest.fixture(scope="module", autouse=True)
-def _native_model():
-    if not (nm.available("f32") and nm.available("f64")):
-        pytest.fail("oracle/_build/libtvl1_gpu_model_{f32,f64}.so missing: run build()")
+def _native_model(cuda_device):
+    if not (nm.available("f32") and nm.available("f64") and nm.available("eng")):
+        pytest.fail("oracle/_build/libtvl1_gpu_model_{f32,f64,eng}.so missing: run build()")
+    nm.set_mufu_tables(*mufu.device_tables(cuda_device))
 
 
 @pytest.fixture(scope="module")
@@ -134,12 +144,14 @@ def test_shape_sweep_vs_native_model(cuda_device, stream, num_sms):
         I0, I1 = _pair(h, w, seed=20 + i, dtype=dtype)
         got, alg = _engine(cuda_device, stream, I0, I1, **SWEEP)
         paths = _check_paths(alg, h, w, P, TVL1_PATH["iter_tma"])
+        exact = nm.calc(I0, I1, P, precision="eng")
         ref = nm.calc(I0, I1, P)
         yard = metrics.epe(ref, nm.calc(I0, I1, P, precision="f64"))
         print(f"sweep {h}x{w} {dtype} ({why}): regions {-(-w // TILE) * -(-h // TILE)} on {num_sms} SMs, "
               f"active path {paths}")
         assert np.isfinite(got).all()
-        _check_vs_yardstick(metrics.epe(got, ref), yard, FLOORS, f"  {h}x{w}")
+        _assert_bits(got, exact, f"{h}x{w}")
+        _check_vs_yardstick(metrics.epe(exact, ref), yard, FLOORS, f"  {h}x{w}")
     print(f"sweep: {time.time() - t0:.1f} s")
 
 
@@ -149,15 +161,18 @@ def test_baseline_size_vs_native_model(cuda_device, stream, h, w):
     I0, I1, _ = synth.make_pair(h, w, seed=0, kind="smooth")
     P = gm.TVL1Params(**BASELINE)
     t0 = time.time()
+    exact = nm.calc(I0, I1, P, precision="eng")
+    t_eng = time.time() - t0
     ref = nm.calc(I0, I1, P)
     yard = metrics.epe(ref, nm.calc(I0, I1, P, precision="f64"))
-    t_model = time.time() - t0
+    t_model = time.time() - t0 - t_eng
+    _check_vs_yardstick(metrics.epe(exact, ref), yard, None, f"{w}x{h} model")
     for path, flags in ((0, TVL1_PATH["iter_tma"]), (1, TVL1_PATH["iter_unfused"])):
         got, alg = _engine(cuda_device, stream, I0, I1, path=path, **BASELINE)
         paths = _check_paths(alg, h, w, P, flags)
         assert np.isfinite(got).all()
-        _check_vs_yardstick(metrics.epe(got, ref), yard, None, f"{w}x{h} path {path} {paths}")
-    print(f"{w}x{h}: model (float + double) {t_model:.1f} s")
+        _assert_bits(got, exact, f"{w}x{h} path {path} {paths}")
+    print(f"{w}x{h}: engine-rounding model {t_eng:.1f} s, float + double model {t_model:.1f} s")
 
 
 def test_staged_window_fallback_multi_wave(cuda_device, stream):
@@ -175,22 +190,27 @@ def test_staged_window_fallback_multi_wave(cuda_device, stream):
         got, alg = _engine(cuda_device, stream, I0, I1, init=init, nscales=1, warps=2, epsilon=0.0, iterations=10,
                            useInitialFlow=True)
         paths = _check_paths(alg, h, w, P, TVL1_PATH["iter_tma"])
-        e = metrics.epe(got, nm.calc(I0, I1, P, init_flow=init))
-        print(f"staged window amp {amp}: active path {paths}, max |dflow| {e.max():.2e}")
-        assert np.isfinite(got).all() and e.max() <= 1e-3, (amp, _worst_tiles(e))
+        exact = nm.calc(I0, I1, P, init_flow=init, precision="eng")
+        e = metrics.epe(exact, nm.calc(I0, I1, P, init_flow=init))
+        print(f"staged window amp {amp}: active path {paths}, model eng-vs-f32 max |dflow| {e.max():.2e}")
+        assert np.isfinite(got).all()
+        _assert_bits(got, exact, f"staged window amp {amp}")
+        assert e.max() <= 1e-3, (amp, _worst_tiles(e))
 
 
 def test_reference_defaults_iteration_trace_1080p(cuda_device, stream):
     """create() defaults (5 scales, 5 warps, epsilon 0.01, up to 300 iterations): the reference's stopping rule runs on
     the GPU as a WHILE conditional node.  The engine reports the total number of inner iterations; it must equal the
-    model's per-warp counts summed.  A difference is only excusable where a sampled error sum lay within 1e-5
-    (relative) of scaledEpsilon, where the engine's rounding may decide the other way."""
+    engine-rounding model's per-warp counts summed, and then the flow is bit for bit the model's.  A difference is only
+    excusable where a sampled error sum lay within 1e-5 (relative) of scaledEpsilon: the device sums its error image
+    in another order than the model, so there it may decide the other way."""
     from opencv_contrib_b200._lib import TVL1_PATH
     h, w = 1080, 1920
     I0, I1, _ = synth.make_pair(h, w, seed=5, kind="smooth")
     P = gm.TVL1Params()
     trace, ratios = [], []
-    ref = nm.calc(I0, I1, P, trace=trace, ratios=ratios)
+    exact = nm.calc(I0, I1, P, trace=trace, ratios=ratios, precision="eng")
+    ref = nm.calc(I0, I1, P)
     yard = metrics.epe(ref, nm.calc(I0, I1, P, precision="f64"))
     got, alg = _engine(cuda_device, stream, I0, I1)
     paths = _check_paths(alg, h, w, P, TVL1_PATH["iter_tma"] | TVL1_PATH["iter_unfused"])
@@ -202,4 +222,5 @@ def test_reference_defaults_iteration_trace_1080p(cuda_device, stream):
     if n_engine != n_model:
         assert closest <= 1e-5, (n_engine, n_model, trace, closest)
     else:
-        _check_vs_yardstick(metrics.epe(got, ref), yard, FLOORS, "defaults 1080p")
+        _assert_bits(got, exact, "defaults 1080p")
+        _check_vs_yardstick(metrics.epe(exact, ref), yard, FLOORS, "defaults 1080p")

@@ -1,7 +1,12 @@
 """GPU parity tests for OpticalFlowDual_TVL1 (through the C ABI via ctypes).
 
 Tolerances (stated -- see DESIGN.md "Parity"):
-  * engine vs the CUDA-semantics numpy model: max |dflow| <= 1e-3 px (gamma = 0);
+  * engine vs the engine-rounding model (oracle/tvl1_gpu_model.c, "eng" build, fed the device's own rcp.approx /
+    sqrt.approx tables): bit for bit, uint32 views compared, every kernel path, gamma, float input, initial flow,
+    the median knob and a staged ladder (one iteration, one fused pass, warps, scales, gamma) that names the stage
+    a mismatch starts at;
+  * the emulation of rcp.approx.ftz / sqrt.approx.ftz behind that model: equal to the device on all 2^32 inputs;
+  * engine vs the CUDA-semantics numpy model: max |dflow| <= 1e-3 px (gamma = 0) as before;
   * engine vs the CPU reference oracle (modules/optflow semantics): >= 95 % of interior pixels
     with EPE <= 0.1 px, mean EPE <= 0.08 px, NCC dissimilarity <= 4e-3
     (reference criteria: test_tvl1optflow.cpp:114-142, test_optflow.cpp:462-465);
@@ -13,9 +18,30 @@ import threading
 import numpy as np
 import pytest
 
-from oracle import synth, metrics, tvl1_cpu, tvl1_gpu_model as gm
+from oracle import mufu, synth, metrics, tvl1_cpu, tvl1_gpu_model as gm, tvl1_gpu_model_native as nm
 
 pytestmark = pytest.mark.gpu
+
+
+@pytest.fixture(scope="module")
+def eng(cuda_device):
+    """The engine-rounding model, fed the tables of this device's rcp.approx / sqrt.approx."""
+    if not nm.available("eng"):
+        pytest.fail("oracle/_build/libtvl1_gpu_model_eng.so missing: run build()")
+    nm.set_mufu_tables(*mufu.device_tables(cuda_device))
+    return nm
+
+
+def _assert_bits(got, ref, label):
+    """Bit-for-bit equality (uint32 views); on failure, how many pixels differ and where the first ones are."""
+    assert got.shape == ref.shape and got.dtype == ref.dtype == np.float32, (label, got.shape, ref.shape, ref.dtype)
+    diff = got.view(np.uint32) != ref.view(np.uint32)
+    if diff.any():
+        ys, xs, cs = np.nonzero(diff)
+        first = [(int(y), int(x), int(c)) for y, x, c in zip(ys[:6], xs[:6], cs[:6])]
+        err = np.abs(got.astype(np.float64) - ref)
+        raise AssertionError(f"{label}: {int(diff.sum())} of {diff.size} values differ, max |d| {float(err.max()):.3e}, "
+                             f"first (y, x, component) {first}")
 
 
 def _run(dev, I0, I1, path=0, fused=0, graph=1, stream=None, init=None, _median=None, aux=0, **kw):
@@ -37,19 +63,78 @@ def _run(dev, I0, I1, path=0, fused=0, graph=1, stream=None, init=None, _median=
 
 
 @pytest.mark.parametrize("h,w,kind,seed", [(120, 160, "const", 0), (243, 317, "smooth", 1), (97, 131, "affine", 2)])
-def test_engine_matches_cuda_semantics_model(cuda_device, h, w, kind, seed):
+def test_engine_matches_cuda_semantics_model(cuda_device, eng, h, w, kind, seed):
     I0, I1, gt = synth.make_pair(h, w, seed=seed, kind=kind)
     kw = dict(nscales=4, warps=3, epsilon=0.0, iterations=20)
-    ref = gm.calc(I0, I1, gm.TVL1Params(**kw))
+    P = gm.TVL1Params(**kw)
+    ref = gm.calc(I0, I1, P)
+    exact = eng.calc(I0, I1, P, precision="eng")
     for path in (1, 2, 0):
         got, alg = _run(cuda_device, I0, I1, path=path, **kw)
+        _assert_bits(got, exact, f"kernel_path {path}")
         st = metrics.epe_stats(got, ref)
         assert np.isfinite(got).all() and st["max"] <= 1e-3, (path, st)
     assert alg.getStats()["launches"] > 0
     for aux in (3,):                                       # separable warp kernel on every level
         alt, _ = _run(cuda_device, I0, I1, aux=aux, **kw)
+        _assert_bits(alt, exact, f"aux_path {aux}")
         st = metrics.epe_stats(alt, ref)
         assert np.isfinite(alt).all() and st["max"] <= 1e-3, ("warp kernel variant", aux, st)
+
+
+# One stage more per step, so that a mismatch names the stage it starts at.  Gamma 1.0 makes fi * gamma exact, so a
+# rounding change in the illumination update shows only at a gamma that is not a power of two: hence 0.7 as well.
+LADDER = {
+    "1x1x1": dict(nscales=1, warps=1, epsilon=0.0, iterations=1),     # the warp and one primal-dual update
+    "1x1x8": dict(nscales=1, warps=1, epsilon=0.0, iterations=8),     # one fused pass
+    "1x2x30": dict(nscales=1, warps=2, epsilon=0.0, iterations=30),   # a second warp, passes of 8 + 8 + 8 + 6
+    "3x2x10": dict(nscales=3, warps=2, epsilon=0.0, iterations=10),   # pyramid resize and flow prolongation
+    "3x2x10-gamma1": dict(nscales=3, warps=2, epsilon=0.0, iterations=10, gamma=1.0),
+    "3x2x10-gamma0.7": dict(nscales=3, warps=2, epsilon=0.0, iterations=10, gamma=0.7),
+}
+
+
+@pytest.mark.parametrize("kw", list(LADDER.values()), ids=list(LADDER))
+def test_staged_ladder_bit_exact(cuda_device, eng, kw):
+    # odd sizes: tiles and warp boxes straddle every image border, levels 203x277 .. 130x177
+    I0, I1, _ = synth.make_pair(203, 277, seed=12, kind="smooth")
+    got, _ = _run(cuda_device, I0, I1, **kw)
+    _assert_bits(got, eng.calc(I0, I1, gm.TVL1Params(**kw), precision="eng"), str(kw))
+
+
+def test_mufu_emulation_exhaustive(cuda_device, eng):
+    """rcp.approx.ftz.f32 and sqrt.approx.ftz.f32 as the library evaluates them (b2f_approx_probe) against the table
+    emulation the engine-rounding model uses, on every one of the 2^32 float bit patterns, in chunks of 2^28: device
+    values, predictions from the tables with integer operations on the device, compared as bits (any NaN equals any
+    NaN).  Then the model's own C emulation against the device on a sample reaching every exponent."""
+    import torch
+    tabs = [torch.from_numpy(t.view(np.int32)).to(cuda_device) for t in mufu.device_tables(cuda_device)]
+    chunk = 1 << 28
+    for op in (mufu.OP_RCP, mufu.OP_SQRT):
+        bad, examples = 0, []
+        for c in range(1 << 4):
+            b = torch.arange(c * chunk, (c + 1) * chunk, dtype=torch.int64, device=cuda_device)
+            bits = (b - ((b >> 31) << 32)).to(torch.int32)  # the same 32 bits as int32
+            del b
+            got = mufu.probe(op, bits.view(torch.float32))
+            pred = mufu.predict(op, bits, *tabs)
+            ok = (got.view(torch.int32) == pred) | (torch.isnan(got) & torch.isnan(pred.view(torch.float32)))
+            n = int((~ok).sum())
+            if n:
+                idx = torch.nonzero(~ok)[:4, 0]
+                examples += [(hex(int(bits[i]) & 0xFFFFFFFF), hex(int(got.view(torch.int32)[i]) & 0xFFFFFFFF),
+                              hex(int(pred[i]) & 0xFFFFFFFF)) for i in idx]
+            bad += n
+            del bits, got, pred, ok
+        assert bad == 0, (("rcp", "sqrt")[op], bad, examples[:8])
+    x = mufu.sample_inputs()
+    xd = torch.from_numpy(x).to(cuda_device)
+    for op in (mufu.OP_RCP, mufu.OP_SQRT):
+        dev = mufu.probe(op, xd).cpu().numpy()
+        emu = eng.mufu_apply(op, x)
+        same = (dev.view(np.uint32) == emu.view(np.uint32)) | (np.isnan(dev) & np.isnan(emu))
+        assert same.all(), (op, x[~same][:8], dev[~same][:8], emu[~same][:8])
+    torch.cuda.empty_cache()
 
 
 @pytest.mark.parametrize("K", [1, 2, 3, 5, 6, 7, 10, 12])
@@ -103,28 +188,43 @@ def test_device_side_convergence_loop_equals_host_loop(cuda_device):
         assert np.array_equal(again, dev)
 
 
-def test_gamma_illumination_path(cuda_device):
-    # gamma != 0 is chaotic (1e-7 input noise moves the model by ~0.1 px at a few pixels), so the
-    # tolerance is statistical
+def test_gamma_illumination_path(cuda_device, eng):
+    # gamma != 0 is chaotic (1e-7 input noise moves the model by ~0.1 px at a few pixels): against the numpy model the
+    # tolerance is statistical, against the engine-rounding model it is bit for bit
     I0, I1, _ = synth.make_pair(120, 160, seed=2, kind="const")
     kw = dict(nscales=3, warps=3, epsilon=0.0, iterations=20, gamma=1.0)
     ref = gm.calc(I0, I1, gm.TVL1Params(**kw))
     got, _ = _run(cuda_device, I0, I1, **kw)
+    _assert_bits(got, eng.calc(I0, I1, gm.TVL1Params(**kw), precision="eng"), "gamma 1.0")
     st = metrics.epe_stats(got, ref)
     assert st["mean"] <= 5e-3 and st["frac_le_0.1"] >= 0.99, st
 
 
-def test_float_input_and_initial_flow(cuda_device):
+def test_float_input_and_initial_flow(cuda_device, eng):
     I0, I1, gt = synth.make_pair(120, 160, seed=5, kind="const", dtype="f32")
     kw = dict(nscales=3, warps=3, epsilon=0.0, iterations=20)
     ref = gm.calc(I0, I1, gm.TVL1Params(**kw))
     got, _ = _run(cuda_device, I0, I1, **kw)
+    _assert_bits(got, eng.calc(I0, I1, gm.TVL1Params(**kw), precision="eng"), "float input")
     assert metrics.epe_stats(got, ref)["max"] <= 1e-3
     init = (gt + 0.25).astype(np.float32)
     kw["useInitialFlow"] = True
     ref = gm.calc(I0, I1, gm.TVL1Params(**kw), init_flow=init)
     got, _ = _run(cuda_device, I0, I1, init=init, **kw)
+    _assert_bits(got, eng.calc(I0, I1, gm.TVL1Params(**kw), init_flow=init, precision="eng"), "initial flow")
     assert metrics.epe_stats(got, ref)["max"] <= 1e-3
+
+
+@pytest.mark.parametrize("median", [(3, 3), (5, 4), (5, 0)])
+def test_median_knob_bit_exact(cuda_device, eng, median):
+    """MEDIAN_FILTERING / MEDIAN_PERIOD against the engine-rounding model's median pass, on the fused kernels (whose
+    passes the median splits) and on the unfused pair; period 0 = once per warp."""
+    I0, I1, _ = synth.make_pair(131, 177, seed=13, kind="smooth")
+    kw = dict(nscales=2, warps=2, epsilon=0.0, iterations=10)
+    exact = eng.calc(I0, I1, gm.TVL1Params(**kw), precision="eng", median=median)
+    for path in (0, 1):
+        got, _ = _run(cuda_device, I0, I1, path=path, _median=median, **kw)
+        _assert_bits(got, exact, f"median {median} kernel_path {path}")
 
 
 def test_tiled_warp_kernel_bit_identical_to_separable(cuda_device):

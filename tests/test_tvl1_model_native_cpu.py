@@ -6,19 +6,34 @@ tests (tests/test_tvl1_fullsize_gpu.py) compare the engine with.
     hypotf) -- do not break bit-equality: the flows below compare as raw bits.
   * The error image is summed in numpy's pairwise order, so the epsilon cadence decides as the numpy model does.
   * The double build is the yardstick for float rounding; its distance from the float build at the GPU tests'
-    small-size configurations is recorded here, and it is what allows the 1e-3 px bound there.
+    small-size configurations is recorded here.
+  * The engine-rounding build ("eng", the model the engine must equal bit for bit): its emulation of rcp.approx /
+    sqrt.approx, fed tables of the correctly rounded operations, is 1/x and sqrt(x) wherever the result is normal and
+    flushes as .ftz says; fed those tables it stays within FACTOR x (float vs double) of the float build, so the
+    engine's departures cannot grow into an error the float yardstick would not allow; and no build's result depends
+    on the OpenMP thread count.  (The device tables, and the emulation against the device on all 2^32 inputs, are
+    tests/test_tvl1_gpu.py's.)
 """
 import numpy as np
 import pytest
 
-from oracle import metrics, synth, tvl1_gpu_model as gm, tvl1_gpu_model_native as nm
+from oracle import metrics, mufu, synth, tvl1_gpu_model as gm, tvl1_gpu_model_native as nm
+
+FACTOR = 4.0  # as in tests/test_tvl1_fullsize_gpu.py
 
 
 @pytest.fixture(scope="module", autouse=True)
 def _built():
-    if not (nm.available("f32") and nm.available("f64")):
+    if not (nm.available("f32") and nm.available("f64") and nm.available("eng")):
         import __graft_entry__ as g
         g.build()
+
+
+@pytest.fixture(scope="module")
+def eng_cr():
+    """The "eng" build fed the correctly rounded tables."""
+    nm.set_mufu_tables(*mufu.correctly_rounded_tables())
+    return nm
 
 
 def _pair(h, w, seed, dtype="u8", kind="smooth"):
@@ -103,3 +118,87 @@ def test_double_build_yardstick_at_small_gpu_test_configs():
         assert b.dtype == np.float64
         e = metrics.epe(a, b)
         assert 0 < e.max() <= 2 * measured and 4 * e.max() <= 1e-3, (h, w, e.max())
+
+
+def test_mufu_emulation_on_correctly_rounded_tables(eng_cr):
+    import torch
+    x = mufu.sample_inputs()
+    with np.errstate(invalid="ignore"):
+        x64 = x.astype(np.float64)
+    bits = x.view(np.uint32)
+    e = (bits >> 23) & 0xFF
+    neg = (bits >> 31) == 1
+    normal_in = (e > 0) & (e < 255)
+    tabs = [torch.from_numpy(t.view(np.int32)) for t in mufu.correctly_rounded_tables()]
+    with np.errstate(divide="ignore", invalid="ignore", over="ignore"):
+        ieee = {mufu.OP_RCP: (1.0 / x64).astype(np.float32), mufu.OP_SQRT: np.sqrt(x64).astype(np.float32)}
+    for op in (mufu.OP_RCP, mufu.OP_SQRT):
+        got = eng_cr.mufu_apply(op, x)
+        # the C emulation and the torch statement of the rule (what the GPU test checks on the device) agree
+        pred = mufu.predict(op, torch.from_numpy(x.view(np.int32)), *tabs).numpy().view(np.float32)
+        same = (got.view(np.uint32) == pred.view(np.uint32)) | (np.isnan(got) & np.isnan(pred))
+        assert same.all(), (op, x[~same][:8])
+        ref = ieee[op]
+        ok = normal_in & (np.abs(ref) >= np.finfo(np.float32).tiny) & np.isfinite(ref)
+        assert ok.sum() > 1_000_000
+        assert np.array_equal(got[ok].view(np.uint32), ref[ok].view(np.uint32)), op
+        zero_in = e == 0
+        if op == mufu.OP_RCP:
+            assert np.array_equal(got[zero_in], np.where(neg[zero_in], -np.inf, np.inf).astype(np.float32))
+            flushed = normal_in & (np.abs(ref) < np.finfo(np.float32).tiny)
+            assert flushed.sum() > 0 and np.all(got[flushed] == 0)
+            assert np.array_equal(np.signbit(got[flushed]), neg[flushed])
+            inf_in = np.isinf(x)
+            assert np.all(got[inf_in] == 0) and np.array_equal(np.signbit(got[inf_in]), neg[inf_in])
+        else:
+            assert np.all(got[zero_in] == 0) and np.array_equal(np.signbit(got[zero_in]), neg[zero_in])
+            assert np.isnan(got[neg & ~zero_in]).all()
+            assert np.isposinf(got[np.isposinf(x)]).all()
+        assert np.isnan(got[np.isnan(x)]).all()
+
+
+@pytest.mark.parametrize("case", ["const", "smooth", "affine", "gamma"])
+def test_engine_rounding_build_within_float_yardstick(eng_cr, case):
+    """With correctly rounded tables, the engine's roundings move the flow no further from the float model than
+    FACTOR x the float model's own distance from the double model, at the small GPU-test configurations."""
+    (h, w, kind, seed), kw = {"const": ((120, 160, "const", 0), SMALL), "smooth": ((243, 317, "smooth", 1), SMALL),
+                              "affine": ((97, 131, "affine", 2), SMALL),
+                              "gamma": ((120, 160, "const", 2), dict(nscales=3, warps=3, epsilon=0.0, iterations=20,
+                                                                     gamma=1.0))}[case]
+    I0, I1, _ = synth.make_pair(h, w, seed=seed, kind=kind)
+    P = gm.TVL1Params(**kw)
+    f32 = nm.calc(I0, I1, P)
+    yard = metrics.epe(f32, nm.calc(I0, I1, P, precision="f64"))
+    e = metrics.epe(nm.calc(I0, I1, P, precision="eng"), f32)
+    for q in (0.5, 0.99, 1.0):
+        v, y = float(np.quantile(e, q)), float(np.quantile(yard, q))
+        assert v <= FACTOR * y, (case, q, v, y)
+
+
+def test_median_knob_in_every_build():
+    """The median pass (MEDIAN_FILTERING 3 / 5 every MEDIAN_PERIOD iterations) is exact selection, so it is not a
+    rounding departure: kernel 1 changes nothing, kernels 3 and 5 change the flow, in every build alike."""
+    I0, I1 = _pair(97, 131, seed=8)
+    P = gm.TVL1Params(nscales=2, warps=2, epsilon=0.0, iterations=10)
+    base = nm.calc(I0, I1, P)
+    assert _bits_equal(base, nm.calc(I0, I1, P, median=(1, 3)))
+    m5 = nm.calc(I0, I1, P, median=(5, 3))
+    assert not np.array_equal(base, m5)
+    assert metrics.epe(m5, nm.calc(I0, I1, P, median=(5, 3), precision="f64")).max() <= 1e-3
+
+
+@pytest.mark.parametrize("precision", ["f32", "eng"])
+def test_result_independent_of_thread_count(eng_cr, precision):
+    I0, I1 = _pair(97, 131, seed=9)
+    P = gm.TVL1Params(nscales=3, warps=2, epsilon=0.01, iterations=30, gamma=0.5)
+    n = nm.set_threads(0, precision)
+    try:
+        runs = []
+        for t in sorted({1, 3, max(n, 2)}):
+            nm.set_threads(t, precision)
+            tr = []
+            runs.append((nm.calc(I0, I1, P, trace=tr, precision=precision, median=(3, 4)), tr))
+    finally:
+        nm.set_threads(n, precision)
+    for flow, tr in runs[1:]:
+        assert _bits_equal(runs[0][0], flow) and tr == runs[0][1]
