@@ -617,6 +617,70 @@ B2F_API void b2f_superres_destroy(b2f_superres *sr);
 B2F_API int b2f_calc_ext(b2f_handle *h, const b2f_image *I0, const b2f_image *I1, b2f_image *flow1, b2f_image *flow2,
                          void *cuda_stream);
 
+/* ---- cudaimgproc corners: cv::cuda::CornernessCriteria and cv::cuda::CornersDetector (modules/cudaimgproc/include/
+ *      opencv2/cudaimgproc.hpp:538-620; src/corners.cpp, src/gftt.cpp, src/cuda/corners.cu, src/cuda/gftt.cu).
+ *   Response (b2f_harris_create / b2f_mineig_create + b2f_corners_compute): src device 8UC1 or 32FC1 (else
+ *      B2F_UNSUPPORTED_TYPE), pitched or an ROI; dst device 32FC1 of the same size.  The derivatives are the reference's
+ *      Sobel (ksize 1, 3, 5, 7) or Scharr (ksize <= 0) filters with scale 1 / (2^(ksize' - 1) blockSize (2 if ksize < 0)
+ *      (255 for 8U)) folded into the smoothing kernel, then the blockSize x blockSize sums of dx^2, dx dy, dy^2 read the
+ *      derivatives through the border rule again.  Harris: a c - b^2 - k (a + c)^2; min-eigenvalue: with a, c halved,
+ *      (a + c) - sqrt((a - c)^2 + b^2).  border_type: 4 BORDER_REFLECT101, 1 BORDER_REPLICATE or 2 BORDER_REFLECT, with
+ *      cudev's rules (one fold and a modulo).  One fused kernel: no intermediate planes; asynchronous on `cuda_stream`
+ *      (a NULL stream ends with a device synchronise).  B2F_BAD_ARG: another border or ksize, a blockSize outside 1..31
+ *      (departure: the reference accepts any; 31 keeps the block-sum halo inside one 32 x 16 tile).
+ *   GoodFeaturesToTrack (b2f_gftt_*): the reference's preconditions (qualityLevel > 0, minDistance >= 0, maxCorners >= 0;
+ *      B2F_BAD_ARG at creation), criterion aperture 3 and BORDER_REFLECT101.  b2f_gftt_detect writes up to `capacity`
+ *      (x, y) float pairs to corners_dev -- integer positions, strongest first, the reference's 1 x N CV_32FC2 -- and N
+ *      to *count_dev (device memory).  capacity must be at least b2f_gftt_capacity.  Departures from the reference:
+ *        - no host synchronisation: the maximum response is folded on the device, candidates are counted, sorted and
+ *          selected on the device; the call is asynchronous and can be captured in a CUDA graph.  The one exception:
+ *          the first detect on a new image size synchronises the stream before it re-lays out the handle's workspace;
+ *          inside a capture that call is refused (B2F_BAD_ARG), so run one detect of that size first;
+ *        - candidates of equal response are ordered by raster index, higher first (CPU cv::goodFeaturesToTrack's
+ *          tie order); the reference's unstable sort leaves it unspecified;
+ *        - when there are more than max(1000, int(0.05 rows cols)) candidates, the first that many in this order are
+ *          kept (the reference keeps whichever its atomics appended first);
+ *        - the maximum that qualityLevel scales ignores the mask, as in the CUDA reference (gftt.cpp:120); CPU
+ *          cv::goodFeaturesToTrack takes it under the mask.
+ *      With minDistance >= 1 the result equals the reference's sequential grid rule (gftt.cpp:147-206) exactly, cell
+ *      cvRound(minDistance) included; it is computed as greedy selection in priority order, in parallel rounds. ---- */
+typedef struct b2f_corners b2f_corners;
+B2F_API int b2f_harris_create(int src_type, int block_size, int ksize, double k, int border_type,
+                              b2f_corners **out);                                                  /* corners.cpp:179-182 */
+B2F_API int b2f_mineig_create(int src_type, int block_size, int ksize, int border_type, b2f_corners **out); /* :184-187 */
+/* CornernessCriteria::compute (cudaimgproc.hpp:566) */
+B2F_API int b2f_corners_compute(b2f_corners *h, const b2f_image *src, b2f_image *dst, void *cuda_stream);
+typedef struct b2f_gftt_params {
+    int max_corners;      /* 1000 (0: no limit) */
+    double quality_level; /* 0.01 */
+    double min_distance;  /* 0.0  */
+    int block_size;       /* 3    */
+    int use_harris;       /* 0    */
+    double harris_k;      /* 0.04 */
+} b2f_gftt_params;
+B2F_API void b2f_gftt_default_params(b2f_gftt_params *p);
+/* createGoodFeaturesToTrackDetector (cudaimgproc.hpp:610-620, gftt.cpp:217-222); NULL params: the defaults */
+B2F_API int b2f_gftt_create(int src_type, const b2f_gftt_params *p, b2f_corners **out);
+/* setMaxCorners / setMinDistance (cudaimgproc.hpp:596-599) and the other create() arguments */
+B2F_API int b2f_gftt_set_params(b2f_corners *h, const b2f_gftt_params *p);
+B2F_API int b2f_gftt_get_params(const b2f_corners *h, b2f_gftt_params *p);
+/* the largest N a detect on a rows x cols image can return: min(maxCorners, max(1000, int(0.05 rows cols))) */
+B2F_API int b2f_gftt_capacity(const b2f_corners *h, int rows, int cols, int *capacity);
+/* CornersDetector::detect (cudaimgproc.hpp:589, gftt.cpp:107-214); mask: device 8UC1 of the image size or NULL */
+B2F_API int b2f_gftt_detect(b2f_corners *h, const b2f_image *image, const b2f_image *mask, float *corners_dev,
+                            int capacity, int *count_dev, void *cuda_stream);
+/* What the last detect did (no reference counterpart): candidates found, candidates kept after the capacity cut, whether
+ * the cut applied, and the rounds of the minDistance selection (0 with minDistance < 1).  Waits for `cuda_stream`. */
+typedef struct b2f_gftt_info {
+    int candidates;
+    int kept;
+    int capped;
+    int rounds;
+} b2f_gftt_info;
+B2F_API int b2f_gftt_last_info(b2f_corners *h, b2f_gftt_info *out, void *cuda_stream);
+B2F_API int b2f_corners_last_cuda_error(const b2f_corners *h);
+B2F_API void b2f_corners_destroy(b2f_corners *h);
+
 #ifdef __cplusplus
 }
 #endif

@@ -11,6 +11,7 @@ Only what the hot path needs lives here:
   frames.py        interpolateFrames, the consumer right after the solvers
   flowio.py        Middlebury .flo files + the reference's error statistics
   superres.py      superres's BTV-L1 video super-resolution and its four CUDA optical-flow wrappers
+  cudaimgproc.py   cudaimgproc's corner responses and GoodFeaturesToTrack detector
 """
 from .cudaoptflow import (  # noqa: F401
     DenseOpticalFlow,
@@ -46,4 +47,11 @@ from .superres import (  # noqa: F401
     createOptFlow_DualTVL1_CUDA,
     createOptFlow_Brox_CUDA,
     createOptFlow_PyrLK_CUDA,
+)
+from .cudaimgproc import (  # noqa: F401
+    CornernessCriteria,
+    CornersDetector,
+    createHarrisCorner,
+    createMinEigenValCorner,
+    createGoodFeaturesToTrackDetector,
 )

@@ -78,6 +78,15 @@ class b2f_superres_params(C.Structure):
                 ("blur_sigma", C.c_double), ("temporal_area_radius", C.c_int)]
 
 
+class b2f_gftt_params(C.Structure):
+    _fields_ = [("max_corners", C.c_int), ("quality_level", C.c_double), ("min_distance", C.c_double),
+                ("block_size", C.c_int), ("use_harris", C.c_int), ("harris_k", C.c_double)]
+
+
+class b2f_gftt_info(C.Structure):
+    _fields_ = [("candidates", C.c_int), ("kept", C.c_int), ("capped", C.c_int), ("rounds", C.c_int)]
+
+
 class b2f_stats(C.Structure):
     _fields_ = [("calls", C.c_uint64), ("launches", C.c_uint64),
                 ("class_launches", C.c_uint64 * B2F_MAX_KERNEL_CLASSES),
@@ -179,6 +188,18 @@ SYMBOLS = [
     ("b2f_superres_last_cuda_error", C.c_int, [_H]),
     ("b2f_superres_destroy", None, [_H]),
     ("b2f_calc_ext", C.c_int, [_H, _IMG, _IMG, _IMG, _IMG, C.c_void_p]),
+    ("b2f_harris_create", C.c_int, [C.c_int, C.c_int, C.c_int, C.c_double, C.c_int, C.POINTER(_H)]),
+    ("b2f_mineig_create", C.c_int, [C.c_int, C.c_int, C.c_int, C.c_int, C.POINTER(_H)]),
+    ("b2f_corners_compute", C.c_int, [_H, _IMG, _IMG, C.c_void_p]),
+    ("b2f_gftt_default_params", None, [C.POINTER(b2f_gftt_params)]),
+    ("b2f_gftt_create", C.c_int, [C.c_int, C.POINTER(b2f_gftt_params), C.POINTER(_H)]),
+    ("b2f_gftt_set_params", C.c_int, [_H, C.POINTER(b2f_gftt_params)]),
+    ("b2f_gftt_get_params", C.c_int, [_H, C.POINTER(b2f_gftt_params)]),
+    ("b2f_gftt_capacity", C.c_int, [_H, C.c_int, C.c_int, C.POINTER(C.c_int)]),
+    ("b2f_gftt_detect", C.c_int, [_H, _IMG, _IMG, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p]),
+    ("b2f_gftt_last_info", C.c_int, [_H, C.POINTER(b2f_gftt_info), C.c_void_p]),
+    ("b2f_corners_last_cuda_error", C.c_int, [_H]),
+    ("b2f_corners_destroy", None, [_H]),
     ("b2f_flo_read_size", C.c_int, [C.c_char_p, C.POINTER(C.c_int), C.POINTER(C.c_int)]),
     ("b2f_flo_read", C.c_int, [C.c_char_p, C.c_void_p, C.c_size_t, C.c_int, C.c_int]),
     ("b2f_flo_write", C.c_int, [C.c_char_p, C.c_void_p, C.c_size_t, C.c_int, C.c_int]),

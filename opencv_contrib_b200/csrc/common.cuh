@@ -108,7 +108,14 @@ struct DeviceScope {
     bool switched = false;
     DeviceScope(const void *device_ptr, cudaStream_t s) {
         int target = -1;
-        if (s != nullptr && s != cudaStreamLegacy && s != cudaStreamPerThread) {
+        // cudaStreamGetDevice on a stream that is being captured fails and invalidates the capture: under capture
+        // the device is taken from the image instead
+        cudaStreamCaptureStatus cap = cudaStreamCaptureStatusNone;
+        if (s != nullptr && s != cudaStreamLegacy && s != cudaStreamPerThread && cudaStreamIsCapturing(s, &cap) != cudaSuccess) {
+            cudaGetLastError();
+            cap = cudaStreamCaptureStatusNone;
+        }
+        if (s != nullptr && s != cudaStreamLegacy && s != cudaStreamPerThread && cap == cudaStreamCaptureStatusNone) {
             if (cudaStreamGetDevice(s, &target) != cudaSuccess) {
                 cudaGetLastError();
                 target = -1;
