@@ -189,9 +189,11 @@ __global__ void __launch_bounds__(256) k_farn_blur_v(Plane f0, Plane f1, int row
         sy = t ? min(y1 + 1, rows - 1) : min(y1, rows - 1);
     }
     const Plane src = blockIdx.z ? f1 : f0;
-    float acc = __ldg(&src.at(sy, x)) * g[0];
+    // a tap chain of run-time length: the centre tap is a plain product, every pair one fused multiply-add
+    float acc = __fmul_rn(__ldg(&src.at(sy, x)), g[0]);
     for (int j = 1; j <= khalf; ++j)
-        acc += (__ldg(&src.at(reflect101(sy - j, rows), x)) + __ldg(&src.at(reflect101(sy + j, rows), x))) * g[j];
+        acc = __fmaf_rn(__fadd_rn(__ldg(&src.at(reflect101(sy - j, rows), x)), __ldg(&src.at(reflect101(sy + j, rows), x))),
+                        g[j], acc);
     (blockIdx.z ? v1 : v0).at(vy, x) = acc;
 }
 
@@ -219,19 +221,22 @@ __global__ void __launch_bounds__(256) k_farn_blur_v4(Plane f0, Plane f1, int ro
     const Plane src = blockIdx.z ? f1 : f0;
     const float4 c = __ldg(reinterpret_cast<const float4 *>(&src.at(sy, x)));
     const float g0 = g[0];
-    float4 acc = make_float4(c.x * g0, c.y * g0, c.z * g0, c.w * g0);
+    float4 acc = make_float4(__fmul_rn(c.x, g0), __fmul_rn(c.y, g0), __fmul_rn(c.z, g0), __fmul_rn(c.w, g0));
     for (int j = 1; j <= khalf; ++j) {
         const float4 a = __ldg(reinterpret_cast<const float4 *>(&src.at(reflect101(sy - j, rows), x)));
         const float4 b = __ldg(reinterpret_cast<const float4 *>(&src.at(reflect101(sy + j, rows), x)));
         const float gj = g[j];
-        acc.x += (a.x + b.x) * gj;
-        acc.y += (a.y + b.y) * gj;
-        acc.z += (a.z + b.z) * gj;
-        acc.w += (a.w + b.w) * gj;
+        acc.x = __fmaf_rn(__fadd_rn(a.x, b.x), gj, acc.x);
+        acc.y = __fmaf_rn(__fadd_rn(a.y, b.y), gj, acc.y);
+        acc.z = __fmaf_rn(__fadd_rn(a.z, b.z), gj, acc.z);
+        acc.w = __fmaf_rn(__fadd_rn(a.w, b.w), gj, acc.w);
     }
     *reinterpret_cast<float4 *>(&(blockIdx.z ? v1 : v0).at(vy, x)) = acc;
 }
 
+// Plain expressions on purpose: written with intrinsics, this chain makes nvcc schedule k_farn_blur_h_resize differently
+// (22 more FFMA, one more register).  The SASS rounds it as k_farn_blur_v does: res = v * g[0], then
+// res = fma(a + b, g[i], res) per pair.
 __device__ __forceinline__ float farn_hblur(const Plane &v, int vy, int sx, int cols, const float *__restrict__ g,
                                             int khalf) {
     float res = v.at(vy, sx) * g[0];
@@ -251,22 +256,30 @@ __global__ void __launch_bounds__(256) k_farn_blur_h_resize(Plane v0, Plane v1, 
     if (identity) {
         out = farn_hblur(v, 2 * y, x, cols, g, khalf);
     } else {
-        const float src_x = x * inv_fx, src_y = y * inv_fy;
+        const float src_x = __fmul_rn(x, inv_fx), src_y = __fmul_rn(y, inv_fy);
         const int x1 = __float2int_rd(src_x), y1 = __float2int_rd(src_y);
         const int x2 = x1 + 1, y2 = y1 + 1;
         const int x1r = min(x1, cols - 1), x2r = min(x2, cols - 1);
         const float wx2 = x2 - src_x, wx1 = src_x - x1;
         const float wy2 = y2 - src_y, wy1 = src_y - y1;
         out = 0.f;
-        // same accumulation order as resize_linear; zero-weight taps add exactly 0 and are skipped
-        out = out + farn_hblur(v, 2 * y, x1r, cols, g, khalf) * (wx2 * wy2);
-        if (wx1 != 0.f) out = out + farn_hblur(v, 2 * y, x2r, cols, g, khalf) * (wx1 * wy2);
+        // same accumulation order and rounding as resize_sample (pyramid.cu): each weight product rounded on its own,
+        // one fused multiply-add per tap onto +0; zero-weight taps would add exactly 0 and are skipped
+        out = __fmaf_rn(farn_hblur(v, 2 * y, x1r, cols, g, khalf), __fmul_rn(wx2, wy2), out);
+        if (wx1 != 0.f) out = __fmaf_rn(farn_hblur(v, 2 * y, x2r, cols, g, khalf), __fmul_rn(wx1, wy2), out);
         if (wy1 != 0.f) {
-            out = out + farn_hblur(v, 2 * y + 1, x1r, cols, g, khalf) * (wx2 * wy1);
-            if (wx1 != 0.f) out = out + farn_hblur(v, 2 * y + 1, x2r, cols, g, khalf) * (wx1 * wy1);
+            out = __fmaf_rn(farn_hblur(v, 2 * y + 1, x1r, cols, g, khalf), __fmul_rn(wx2, wy1), out);
+            if (wx1 != 0.f) out = __fmaf_rn(farn_hblur(v, 2 * y + 1, x2r, cols, g, khalf), __fmul_rn(wx1, wy1), out);
         }
     }
     (blockIdx.z ? d1 : d0).at(y, x) = out;
+}
+
+// One step k >= 1 of an unrolled symmetric tap chain c * g[0] + sum_k s_k * g[k]: the centre product rounds on its own
+// only where nvcc cannot fuse it, so the first step is fma(c, g[0], s_1 * g[1]) and every later one fma(s_k, g[k], acc).
+// This is the instruction sequence nvcc contracts the plain chain into when the length is known at compile time.
+__device__ __forceinline__ float farn_tap(int k, float c, const float *g, float s, float acc) {
+    return k == 1 ? __fmaf_rn(c, g[0], __fmul_rn(s, g[1])) : __fmaf_rn(s, g[k], acc);
 }
 
 // ------------------------------------------------------------------------------------------
@@ -286,6 +299,8 @@ __global__ void __launch_bounds__(256) k_farn_polyexp(Plane s0, Plane s1, Stack5
     if (y < rows) {
         for (int i = tx; i < SW; i += TW) {
             const int xc = clampi(x0 + i - N, 0, cols - 1);
+            // plain on purpose (intrinsics here cost a register); the SASS is farn_tap's sequence for a0 and
+            // fma(xg[k], t1 - t0, a1), fma(xxg[k], t0 + t1, a2) from +0
             float a0 = __ldg(&src.at(y, xc)) * T.g[0], a1 = 0.f, a2 = 0.f;
 #pragma unroll
             for (int k = 1; k <= N; ++k) {
@@ -304,22 +319,21 @@ __global__ void __launch_bounds__(256) k_farn_polyexp(Plane s0, Plane s1, Stack5
     const int x = x0 + tx;
     if (y >= rows || x >= cols) return;
     const float *row0 = &sm[0][ty][tx + N], *row1 = &sm[1][ty][tx + N], *row2 = &sm[2][ty][tx + N];
-    float b1 = T.g[0] * row0[0], b3 = T.g[0] * row1[0], b5 = T.g[0] * row2[0];
-    float b2 = 0.f, b4 = 0.f, b6 = 0.f;
+    float b1 = 0.f, b2 = 0.f, b3 = 0.f, b4 = 0.f, b5 = 0.f, b6 = 0.f;
 #pragma unroll
     for (int k = 1; k <= N; ++k) {
-        b1 += (row0[k] + row0[-k]) * T.g[k];
-        b4 += (row0[k] + row0[-k]) * T.xxg[k];
-        b2 += (row0[k] - row0[-k]) * T.xg[k];
-        b3 += (row1[k] + row1[-k]) * T.g[k];
-        b6 += (row1[k] - row1[-k]) * T.xg[k];
-        b5 += (row2[k] + row2[-k]) * T.g[k];
+        b1 = farn_tap(k, row0[0], T.g, __fadd_rn(row0[k], row0[-k]), b1);
+        b4 = __fmaf_rn(__fadd_rn(row0[k], row0[-k]), T.xxg[k], b4);
+        b2 = __fmaf_rn(__fsub_rn(row0[k], row0[-k]), T.xg[k], b2);
+        b3 = farn_tap(k, row1[0], T.g, __fadd_rn(row1[k], row1[-k]), b3);
+        b6 = __fmaf_rn(__fsub_rn(row1[k], row1[-k]), T.xg[k], b6);
+        b5 = farn_tap(k, row2[0], T.g, __fadd_rn(row2[k], row2[-k]), b5);
     }
-    dst.at(0, y, x) = b3 * T.ig11;
-    dst.at(1, y, x) = b2 * T.ig11;
-    dst.at(2, y, x) = b1 * T.ig03 + b5 * T.ig33;
-    dst.at(3, y, x) = b1 * T.ig03 + b4 * T.ig33;
-    dst.at(4, y, x) = b6 * T.ig55;
+    dst.at(0, y, x) = __fmul_rn(b3, T.ig11);
+    dst.at(1, y, x) = __fmul_rn(b2, T.ig11);
+    dst.at(2, y, x) = __fmaf_rn(b1, T.ig03, __fmul_rn(b5, T.ig33));
+    dst.at(3, y, x) = __fmaf_rn(b1, T.ig03, __fmul_rn(b4, T.ig33));
+    dst.at(4, y, x) = __fmul_rn(b6, T.ig55);
 }
 
 // Register-blocked variant (the default): in the kernel above every output of the vertical pass issues its own 2N+1
@@ -358,6 +372,8 @@ __global__ void __launch_bounds__(256) k_farn_polyexp_fast(Plane s0, Plane s1, S
         }
 #pragma unroll
         for (int o = 0; o < SEG; ++o) {
+            // plain on purpose, as in k_farn_polyexp: the SASS is farn_tap's sequence for a0 and fma(xg[k], t1 - t0, a1),
+            // fma(xxg[k], t0 + t1, a2) from +0
             float a0 = v[o + N] * T.g[0], a1 = 0.f, a2 = 0.f;
 #pragma unroll
             for (int k = 1; k <= N; ++k) {
@@ -392,6 +408,10 @@ __global__ void __launch_bounds__(256) k_farn_polyexp_fast(Plane s0, Plane s1, S
 #pragma unroll
         for (int e = 0; e < 4; ++e) {
             const int c = e + N;
+            // Plain on purpose: with intrinsics, even for the five outputs alone, this kernel drops from 60 to 58
+            // registers.  The SASS rounds exactly as k_farn_polyexp writes it out: b1, b3, b5 by farn_tap, b2, b4, b6
+            // by fma(sum or difference, table, acc) from +0, and o2 / o3 = fma(b1, ig03, b5 * ig33) / fma(b1, ig03,
+            // b4 * ig33).
             float b1 = T.g[0] * w0[c], b3 = T.g[0] * w1[c], b5 = T.g[0] * w2[c];
             float b2 = 0.f, b4 = 0.f, b6 = 0.f;
 #pragma unroll
@@ -435,9 +455,36 @@ __device__ __forceinline__ float farn_border_w(int d) {
     return d <= 1 ? 0.14f : (d < BORDER_SIZE ? 0.4472f : 1.f);
 }
 
+// a00 t00 + a01 t01 + a10 t10 + a11 t11 as nvcc contracts it: the second product rounds, the others are fused in order
+__device__ __forceinline__ float farn_bilinear(float a00, float a01, float a10, float a11, float t00, float t01, float t10,
+                                               float t11) {
+    return __fmaf_rn(a11, t11, __fmaf_rn(a10, t10, __fmaf_rn(a00, t00, __fmul_rn(a01, t01))));
+}
+
+// The tail of updateMatrices shared by the per-pixel, quad and spread forms, from R0 planes 0 / 1 at the pixel, the
+// gathered (or zero) r2, r3 and the averaged r4, r5, r6:
+//   r2 = (R0_0 - r2) * 0.5 + (r4 dy + r6 dx),  r3 = (R0_1 - r3) * 0.5 + (r6 dy + r5 dx),  then everything * scale.
+// Written as nvcc contracts the plain expressions: the * 0.5 fuses into the outer add, r4 dy is fused onto r6 dx but
+// r5 dx onto r6 dy (nvcc fuses the SECOND product there), and each product pair of M fuses its first product.
+__device__ __forceinline__ void farn_matrices(float r0_0, float r0_1, float r2, float r3, float r4, float r5, float r6,
+                                              float dx, float dy, float scale, float (&m)[5]) {
+    r2 = __fmaf_rn(__fsub_rn(r0_0, r2), 0.5f, __fmaf_rn(r4, dy, __fmul_rn(r6, dx)));
+    r3 = __fmaf_rn(__fsub_rn(r0_1, r3), 0.5f, __fmaf_rn(r5, dx, __fmul_rn(r6, dy)));
+    r2 = __fmul_rn(r2, scale);
+    r3 = __fmul_rn(r3, scale);
+    r4 = __fmul_rn(r4, scale);
+    r5 = __fmul_rn(r5, scale);
+    r6 = __fmul_rn(r6, scale);
+    m[0] = __fmaf_rn(r4, r4, __fmul_rn(r6, r6));
+    m[1] = __fmul_rn(__fadd_rn(r4, r5), r6);
+    m[2] = __fmaf_rn(r5, r5, __fmul_rn(r6, r6));
+    m[3] = __fmaf_rn(r4, r2, __fmul_rn(r6, r3));
+    m[4] = __fmaf_rn(r6, r2, __fmul_rn(r5, r3));
+}
+
 __device__ __forceinline__ void farn_update_matrices_px(const Stack5 &R0, const Stack5 &R1, int rows, int cols, int x,
                                                         int y, float dx, float dy, float (&m)[5]) {
-    float fx = x + dx, fy = y + dy;
+    float fx = __fadd_rn(x, dx), fy = __fadd_rn(y, dy);
     // floorf of a wild flow must not overflow the int conversion
     const float ffx = fminf(fmaxf(floorf(fx), -4.f), (float)cols + 4.f);
     const float ffy = fminf(fmaxf(floorf(fy), -4.f), (float)rows + 4.f);
@@ -451,15 +498,15 @@ __device__ __forceinline__ void farn_update_matrices_px(const Stack5 &R0, const 
         const float *p = &R1.at(0, y1, x1);
         const size_t ps = (size_t)R1.h * R1.pitch;
         const int pitch = R1.pitch;
-        r2 = a00 * __ldg(p) + a01 * __ldg(p + 1) + a10 * __ldg(p + pitch) + a11 * __ldg(p + pitch + 1);
+        r2 = farn_bilinear(a00, a01, a10, a11, __ldg(p), __ldg(p + 1), __ldg(p + pitch), __ldg(p + pitch + 1));
         p += ps;
-        r3 = a00 * __ldg(p) + a01 * __ldg(p + 1) + a10 * __ldg(p + pitch) + a11 * __ldg(p + pitch + 1);
+        r3 = farn_bilinear(a00, a01, a10, a11, __ldg(p), __ldg(p + 1), __ldg(p + pitch), __ldg(p + pitch + 1));
         p += ps;
-        r4 = a00 * __ldg(p) + a01 * __ldg(p + 1) + a10 * __ldg(p + pitch) + a11 * __ldg(p + pitch + 1);
+        r4 = farn_bilinear(a00, a01, a10, a11, __ldg(p), __ldg(p + 1), __ldg(p + pitch), __ldg(p + pitch + 1));
         p += ps;
-        r5 = a00 * __ldg(p) + a01 * __ldg(p + 1) + a10 * __ldg(p + pitch) + a11 * __ldg(p + pitch + 1);
+        r5 = farn_bilinear(a00, a01, a10, a11, __ldg(p), __ldg(p + 1), __ldg(p + pitch), __ldg(p + pitch + 1));
         p += ps;
-        r6 = a00 * __ldg(p) + a01 * __ldg(p + 1) + a10 * __ldg(p + pitch) + a11 * __ldg(p + pitch + 1);
+        r6 = farn_bilinear(a00, a01, a10, a11, __ldg(p), __ldg(p + 1), __ldg(p + pitch), __ldg(p + pitch + 1));
         r4 = (__ldg(&R0.at(2, y, x)) + r4) * 0.5f;
         r5 = (__ldg(&R0.at(3, y, x)) + r5) * 0.5f;
         r6 = (__ldg(&R0.at(4, y, x)) + r6) * 0.25f;
@@ -469,18 +516,9 @@ __device__ __forceinline__ void farn_update_matrices_px(const Stack5 &R0, const 
         r5 = __ldg(&R0.at(3, y, x));
         r6 = __ldg(&R0.at(4, y, x)) * 0.5f;
     }
-    r2 = (__ldg(&R0.at(0, y, x)) - r2) * 0.5f;
-    r3 = (__ldg(&R0.at(1, y, x)) - r3) * 0.5f;
-    r2 += r4 * dy + r6 * dx;
-    r3 += r6 * dy + r5 * dx;
     const float scale = farn_border_w(min(x, BORDER_SIZE)) * farn_border_w(min(y, BORDER_SIZE)) *
                         farn_border_w(min(cols - x - 1, BORDER_SIZE)) * farn_border_w(min(rows - y - 1, BORDER_SIZE));
-    r2 *= scale; r3 *= scale; r4 *= scale; r5 *= scale; r6 *= scale;
-    m[0] = r4 * r4 + r6 * r6;
-    m[1] = (r4 + r5) * r6;
-    m[2] = r5 * r5 + r6 * r6;
-    m[3] = r4 * r2 + r6 * r3;
-    m[4] = r6 * r2 + r5 * r3;
+    farn_matrices(__ldg(&R0.at(0, y, x)), __ldg(&R0.at(1, y, x)), r2, r3, r4, r5, r6, dx, dy, scale, m);
 }
 
 
@@ -495,7 +533,7 @@ __device__ __forceinline__ void farn_update_matrices_quad(const Stack5 &R0, cons
     bool inb[4];
 #pragma unroll
     for (int e = 0; e < 4; ++e) {
-        float fx = (x + e) + dx[e], fy = y + dy[e];
+        float fx = __fadd_rn(x + e, dx[e]), fy = __fadd_rn(y, dy[e]);
         const float ffx = fminf(fmaxf(floorf(fx), -4.f), (float)cols + 4.f);
         const float ffy = fminf(fmaxf(floorf(fy), -4.f), (float)rows + 4.f);
         const int x1 = (int)ffx, y1 = (int)ffy;
@@ -525,7 +563,7 @@ __device__ __forceinline__ void farn_update_matrices_quad(const Stack5 &R0, cons
             base[e] = p + ps;  // next plane
         }
 #pragma unroll
-        for (int e = 0; e < 4; ++e) g[k][e] = a00[e] * t00[e] + a01[e] * t01[e] + a10[e] * t10[e] + a11[e] * t11[e];
+        for (int e = 0; e < 4; ++e) g[k][e] = farn_bilinear(a00[e], a01[e], a10[e], a11[e], t00[e], t01[e], t10[e], t11[e]);
     }
     float r0v[5][4];
     const bool full = x + 3 < cols;
@@ -554,19 +592,10 @@ __device__ __forceinline__ void farn_update_matrices_quad(const Stack5 &R0, cons
             r5 = r0v[3][e];
             r6 = r0v[4][e] * 0.5f;
         }
-        r2 = (r0v[0][e] - r2) * 0.5f;
-        r3 = (r0v[1][e] - r3) * 0.5f;
-        r2 += r4 * dy[e] + r6 * dx[e];
-        r3 += r6 * dy[e] + r5 * dx[e];
         const int xe = x + e;
         const float scale = farn_border_w(min(xe, BORDER_SIZE)) * farn_border_w(min(y, BORDER_SIZE)) *
                             farn_border_w(min(cols - xe - 1, BORDER_SIZE)) * farn_border_w(min(rows - y - 1, BORDER_SIZE));
-        r2 *= scale; r3 *= scale; r4 *= scale; r5 *= scale; r6 *= scale;
-        m[e][0] = r4 * r4 + r6 * r6;
-        m[e][1] = (r4 + r5) * r6;
-        m[e][2] = r5 * r5 + r6 * r6;
-        m[e][3] = r4 * r2 + r6 * r3;
-        m[e][4] = r6 * r2 + r5 * r3;
+        farn_matrices(r0v[0][e], r0v[1][e], r2, r3, r4, r5, r6, dx[e], dy[e], scale, m[e]);
     }
 }
 
@@ -584,7 +613,7 @@ __device__ __forceinline__ void farn_update_matrices_spread(const Stack5 &R0, co
     bool inb[4];
 #pragma unroll
     for (int e = 0; e < 4; ++e) {
-        float fx = xs[e] + dx[e], fy = ys[e] + dy[e];
+        float fx = __fadd_rn(xs[e], dx[e]), fy = __fadd_rn(ys[e], dy[e]);
         const float ffx = fminf(fmaxf(floorf(fx), -4.f), (float)cols + 4.f);
         const float ffy = fminf(fmaxf(floorf(fy), -4.f), (float)rows + 4.f);
         const int x1 = (int)ffx, y1 = (int)ffy;
@@ -614,7 +643,7 @@ __device__ __forceinline__ void farn_update_matrices_spread(const Stack5 &R0, co
             base[e] = p + ps;  // next plane
         }
 #pragma unroll
-        for (int e = 0; e < 4; ++e) g[k][e] = a00[e] * t00[e] + a01[e] * t01[e] + a10[e] * t10[e] + a11[e] * t11[e];
+        for (int e = 0; e < 4; ++e) g[k][e] = farn_bilinear(a00[e], a01[e], a10[e], a11[e], t00[e], t01[e], t10[e], t11[e]);
     }
     float r0v[5][4];
 #pragma unroll
@@ -636,20 +665,20 @@ __device__ __forceinline__ void farn_update_matrices_spread(const Stack5 &R0, co
             r5 = r0v[3][e];
             r6 = r0v[4][e] * 0.5f;
         }
-        r2 = (r0v[0][e] - r2) * 0.5f;
-        r3 = (r0v[1][e] - r3) * 0.5f;
-        r2 += r4 * dy[e] + r6 * dx[e];
-        r3 += r6 * dy[e] + r5 * dx[e];
         const int xe = xs[e], ye = ys[e];
         const float scale = farn_border_w(min(xe, BORDER_SIZE)) * farn_border_w(min(ye, BORDER_SIZE)) *
                             farn_border_w(min(cols - xe - 1, BORDER_SIZE)) * farn_border_w(min(rows - ye - 1, BORDER_SIZE));
-        r2 *= scale; r3 *= scale; r4 *= scale; r5 *= scale; r6 *= scale;
-        m[e][0] = r4 * r4 + r6 * r6;
-        m[e][1] = (r4 + r5) * r6;
-        m[e][2] = r5 * r5 + r6 * r6;
-        m[e][3] = r4 * r2 + r6 * r3;
-        m[e][4] = r6 * r2 + r5 * r3;
+        farn_matrices(r0v[0][e], r0v[1][e], r2, r3, r4, r5, r6, dx[e], dy[e], scale, m[e]);
     }
+}
+
+// updateFlow (farneback.cu:267-286): det = g11 g22 - g12^2 + 1e-3, fx = (g11 h2 - g12 h1) / det, fy = (g22 h1 - g12 h2) / det
+// with the reciprocal taken once, as nvcc contracts the plain expressions: each difference of products fuses its first
+// product onto the negated second; 1.f / d is the IEEE-rounded reciprocal.
+__device__ __forceinline__ void farn_update_flow(float g11, float g12, float g22, float h1, float h2, float &fx, float &fy) {
+    const float detInv = 1.f / __fadd_rn(__fmaf_rn(g11, g22, -__fmul_rn(g12, g12)), 1e-3f);
+    fx = __fmul_rn(__fmaf_rn(g11, h2, -__fmul_rn(g12, h1)), detInv);
+    fy = __fmul_rn(__fmaf_rn(g22, h1, -__fmul_rn(g12, h2)), detInv);
 }
 
 __global__ void __launch_bounds__(256) k_farn_update_matrices(Plane flowx, Plane flowy, Stack5 R0, Stack5 R1, Stack5 M,
@@ -693,7 +722,7 @@ __global__ void __launch_bounds__(256) k_farn_iter(Stack5 Min, Stack5 Mout, Stac
 #pragma unroll
         for (int k = 0; k < 5; ++k) {
             const float c = __ldg(&Min.at(k, y, xc));
-            acc[k] = GAUSS ? c * g[0] : c;
+            acc[k] = GAUSS ? __fmul_rn(c, g[0]) : c;
         }
         for (int j = 1; j <= khalf; ++j) {
             const int ya = max(y - j, 0), yb = min(y + j, rows - 1);
@@ -701,7 +730,7 @@ __global__ void __launch_bounds__(256) k_farn_iter(Stack5 Min, Stack5 Mout, Stac
 #pragma unroll
             for (int k = 0; k < 5; ++k) {
                 const float s = __ldg(&Min.at(k, ya, xc)) + __ldg(&Min.at(k, yb, xc));
-                acc[k] = GAUSS ? acc[k] + s * gj : acc[k] + s;
+                acc[k] = GAUSS ? __fmaf_rn(s, gj, acc[k]) : acc[k] + s;
             }
         }
 #pragma unroll
@@ -719,15 +748,15 @@ __global__ void __launch_bounds__(256) k_farn_iter(Stack5 Min, Stack5 Mout, Stac
 #pragma unroll
         for (int k = 0; k < 5; ++k) {
             const float *row = &sm[(k * IT_TH + r) * sw + lx + khalf];
-            float a = GAUSS ? row[0] * g[0] : row[0];
-            for (int i = 1; i <= khalf; ++i) a = GAUSS ? a + (row[-i] + row[i]) * g[i] : a + (row[-i] + row[i]);
+            // a tap chain of run-time length: the centre tap is a plain product, every pair one fused multiply-add
+            float a = GAUSS ? __fmul_rn(row[0], g[0]) : row[0];
+            for (int i = 1; i <= khalf; ++i)
+                a = GAUSS ? __fmaf_rn(__fadd_rn(row[-i], row[i]), g[i], a) : a + (row[-i] + row[i]);
             res[k] = GAUSS ? a : a * box_inv;
         }
         // updateFlow
-        const float g11 = res[0], g12 = res[1], g22 = res[2], h1 = res[3], h2 = res[4];
-        const float detInv = 1.f / (g11 * g22 - g12 * g12 + 1e-3f);
-        const float fx = (g11 * h2 - g12 * h1) * detInv;
-        const float fy = (g22 * h1 - g12 * h2) * detInv;
+        float fx, fy;
+        farn_update_flow(res[0], res[1], res[2], res[3], res[4], fx, fy);
         if (write_flow) {
             flowx.at(y, x) = fx;
             flowy.at(y, x) = fy;
@@ -744,8 +773,10 @@ __global__ void __launch_bounds__(256) k_farn_iter(Stack5 Min, Stack5 Mout, Stac
 
 // ------------------------------------------------------------------------------------------
 // Register-blocked variant of the fused iteration for a compile-time window half-size K
-// (winSize = 2K+1; K = 6 is the reference default 13).  Same arithmetic and summation order as
-// k_farn_iter, ~4x fewer instructions:
+// (winSize = 2K+1; K = 6 is the reference default 13).  Same arithmetic as k_farn_iter, ~4x fewer instructions,
+// but not the same rounding: the box window is summed as a balanced tree over its first 13 values and then slid with
+// acc + (new - old), restarting at every 16-row strip and every 4-pixel task, and the unrolled gaussian chain lets nvcc
+// fuse the centre tap into the first pair (oracle/farneback_model.c restates both orders):
 //   vertical pass   one task = (column, plane, 16-row half): 16+2K loads feed 16 outputs from a
 //                   register window instead of 2K+1 loads per output;
 //   horizontal pass one task = (row, 4 consecutive pixels): 4 LDS.128 per plane feed 4 outputs;
@@ -804,9 +835,9 @@ __global__ void __launch_bounds__(NT, MINB) k_farn_iter_fast(Stack5 Min, Stack5 
         if (GAUSS) {
 #pragma unroll
             for (int o = 0; o < HALF; ++o) {
-                float acc = v[o + K] * gk[0];
+                float acc = 0.f;
 #pragma unroll
-                for (int j = 1; j <= K; ++j) acc = acc + (v[o + K - j] + v[o + K + j]) * gk[j];
+                for (int j = 1; j <= K; ++j) acc = farn_tap(j, v[o + K], gk, __fadd_rn(v[o + K - j], v[o + K + j]), acc);
                 dst[o * SW] = acc;
             }
         } else {
@@ -846,9 +877,9 @@ __global__ void __launch_bounds__(NT, MINB) k_farn_iter_fast(Stack5 Min, Stack5 
             if (GAUSS) {
 #pragma unroll
                 for (int e = 0; e < 4; ++e) {
-                    float acc = w[e + K] * gk[0];
+                    float acc = 0.f;
 #pragma unroll
-                    for (int i = 1; i <= K; ++i) acc = acc + (w[e + K - i] + w[e + K + i]) * gk[i];
+                    for (int i = 1; i <= K; ++i) acc = farn_tap(i, w[e + K], gk, __fadd_rn(w[e + K - i], w[e + K + i]), acc);
                     res[pl][e] = acc;
                 }
             } else {
@@ -864,10 +895,7 @@ __global__ void __launch_bounds__(NT, MINB) k_farn_iter_fast(Stack5 Min, Stack5 
         float fx[4], fy[4];
 #pragma unroll
         for (int e = 0; e < 4; ++e) {
-            const float g11 = res[0][e], g12 = res[1][e], g22 = res[2][e], h1 = res[3][e], h2 = res[4][e];
-            const float detInv = 1.f / (g11 * g22 - g12 * g12 + 1e-3f);
-            fx[e] = (g11 * h2 - g12 * h1) * detInv;
-            fy[e] = (g22 * h1 - g12 * h2) * detInv;
+            farn_update_flow(res[0][e], res[1][e], res[2][e], res[3][e], res[4][e], fx[e], fy[e]);
         }
         const bool full = x + 3 < cols;
         if (write_flow && live) {
@@ -943,7 +971,7 @@ __global__ void __launch_bounds__(NT, MINB) k_farn_iter_fast(Stack5 Min, Stack5 
 // sums are formed the NEXT tile's boxes are requested into the same buffer and land while this tile runs its
 // horizontal pass, solve and R1 gather.  TMA zero-fills outside the tensor, the blur needs replicate borders:
 // border tiles patch their halo cells from the clamped in-tile position before the vertical pass.
-// Same arithmetic and summation order as k_farn_iter_fast -> bit-identical.
+// Same arithmetic, strip / task geometry and summation order as k_farn_iter_fast -> bit-identical.
 // ------------------------------------------------------------------------------------------
 constexpr int TT = 64;              // tile edge
 constexpr int TB_W = TT + 16;       // box columns: x0-8 .. x0+71 (origin a multiple of 4 floats)
@@ -1041,9 +1069,9 @@ __global__ void __launch_bounds__(TNT, 1)
             if (GAUSS) {
 #pragma unroll
                 for (int o = 0; o < 16; ++o) {
-                    float acc = v[o + K] * gk[0];
+                    float acc = 0.f;
 #pragma unroll
-                    for (int j = 1; j <= K; ++j) acc = acc + (v[o + K - j] + v[o + K + j]) * gk[j];
+                    for (int j = 1; j <= K; ++j) acc = farn_tap(j, v[o + K], gk, __fadd_rn(v[o + K - j], v[o + K + j]), acc);
                     dst[o * TSW] = acc;
                 }
             } else {
@@ -1086,9 +1114,9 @@ __global__ void __launch_bounds__(TNT, 1)
                 if (GAUSS) {
 #pragma unroll
                     for (int e = 0; e < 4; ++e) {
-                        float acc = w[e + K] * gk[0];
+                        float acc = 0.f;
 #pragma unroll
-                        for (int i = 1; i <= K; ++i) acc = acc + (w[e + K - i] + w[e + K + i]) * gk[i];
+                        for (int i = 1; i <= K; ++i) acc = farn_tap(i, w[e + K], gk, __fadd_rn(w[e + K - i], w[e + K + i]), acc);
                         res[pl][e] = acc;
                     }
                 } else {
@@ -1104,10 +1132,7 @@ __global__ void __launch_bounds__(TNT, 1)
             float fx[4], fy[4];
 #pragma unroll
             for (int e = 0; e < 4; ++e) {
-                const float g11 = res[0][e], g12 = res[1][e], g22 = res[2][e], h1 = res[3][e], h2 = res[4][e];
-                const float detInv = 1.f / (g11 * g22 - g12 * g12 + 1e-3f);
-                fx[e] = (g11 * h2 - g12 * h1) * detInv;
-                fy[e] = (g22 * h1 - g12 * h2) * detInv;
+                farn_update_flow(res[0][e], res[1][e], res[2][e], res[3][e], res[4][e], fx[e], fy[e]);
             }
             const bool full = x + 3 < cols;
             if (write_flow) {

@@ -14,6 +14,8 @@
 #include <omp.h>
 #endif
 
+#include "pyr_tap5.h"
+
 enum { MAX_WIN = 256 }; /* the engine's 200 KB patch limit allows windows up to 115 */
 enum { C_WRAPPED, C_SINGULAR, C_LEFT, C_CAPPED, C_CHAIN, N_COUNTERS };
 
@@ -29,46 +31,10 @@ int denselk_model_set_threads(int n) {
 
 int denselk_model_n_counters(void) { return N_COUNTERS; }
 
-static int reflect101(int i, int n) {
-    if (n == 1) return 0;
-    while (i < 0 || i >= n) {
-        if (i < 0) i = -i;
-        if (i >= n) i = 2 * n - 2 - i;
-    }
-    return i;
-}
-
 static int clampi(int v, int lo, int hi) { return v < lo ? lo : (v > hi ? hi : v); }
 
-/* pyramid.cu pyr_tap5 */
-static float tap5(float a, float b, float c, float d, float e) {
-    float s = fmaf(a, 0.0625f, b * 0.25f);
-    s = fmaf(c, 0.375f, s);
-    s = fmaf(d, 0.25f, s);
-    return fmaf(e, 0.0625f, s);
-}
-
-/* k_pyr_down<false>: vertical 5-tap per source column, then horizontal, REFLECT101 */
-void denselk_model_pyr_down(const float *src, int h, int w, float *dst) {
-    const int dh = (h + 1) / 2, dw = (w + 1) / 2;
-    float *V = (float *)malloc(sizeof(float) * (size_t)dh * w);
-#pragma omp parallel for schedule(static)
-    for (int y = 0; y < dh; ++y) {
-        const float *r[5];
-        for (int k = 0; k < 5; ++k) r[k] = src + (size_t)reflect101(2 * y - 2 + k, h) * w;
-        for (int x = 0; x < w; ++x) V[(size_t)y * w + x] = tap5(r[0][x], r[1][x], r[2][x], r[3][x], r[4][x]);
-    }
-#pragma omp parallel for schedule(static)
-    for (int y = 0; y < dh; ++y) {
-        const float *v = V + (size_t)y * w;
-        for (int x = 0; x < dw; ++x) {
-            int rx[5];
-            for (int k = 0; k < 5; ++k) rx[k] = reflect101(2 * x - 2 + k, w);
-            dst[(size_t)y * dw + x] = tap5(v[rx[0]], v[rx[1]], v[rx[2]], v[rx[3]], v[rx[4]]);
-        }
-    }
-    free(V);
-}
+/* k_pyr_down<false> (pyr_tap5.h, shared with farneback_model.c) */
+void denselk_model_pyr_down(const float *src, int h, int w, float *dst) { (void)pyr_tap5_down(src, h, w, dst); }
 
 /* denselk.cu lk_scharr3 */
 static float scharr3(float a, float b, float c) { return fmaf(c, 3.f, fmaf(a, 3.f, 10.f * b)); }

@@ -2,7 +2,7 @@
 (modules/cudaoptflow/src/farneback.cpp + src/cuda/farneback.cu + cudawarping resize/pyrDown).
 
 TEST INFRASTRUCTURE (see oracle/__init__.py).  The parity anchor for Farneback is the LIVE CPU
-reference ``cv2.calcOpticalFlowFarneback`` (oracle/farneback_cpu.py, pinned); this model restates
+reference ``cv2.calcOpticalFlowFarneback`` (pinned in tests/test_oracle_cpu.py); this model restates
 the CUDA reference's stage semantics (top-left resize, 5-plane stacked R/M, border weights,
 replicate-border box filter) so individual kernels can be checked stage by stage.  It cannot be
 pinned against the CUDA reference itself (no GPU OpenCV build) -- the end-to-end check against

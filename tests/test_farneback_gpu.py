@@ -4,7 +4,8 @@ Parity anchor: the LIVE CPU reference cv2.calcOpticalFlowFarneback (opencv/openc
 the function modules/optflow/src/interfaces.cpp:154-157 forwards to), with the reference test's own
 criteria (test_optflow.cpp:341-348): NCC dissimilarity <= 1e-4 (box) / 2e-2 (gaussian), plus a
 mean-EPE bound, and committed golden fixtures (tests/golden/farneback_*.npz, made by
-tests/golden/make_golden.py from cv2) so the check does not depend on the box's cv2.
+tests/golden/make_golden.py from cv2) so the check does not depend on the box's cv2.  Against the model of the
+engine's own roundings (oracle/farneback_model.c) the comparison is exact.
 """
 import os
 
@@ -12,7 +13,7 @@ import numpy as np
 import cv2
 import pytest
 
-from oracle import synth, metrics, farneback_gpu_model as fm
+from oracle import synth, metrics, farneback_gpu_model as fm, farneback_model_native as fn
 
 pytestmark = pytest.mark.gpu
 GOLD = os.path.join(os.path.dirname(__file__), "golden")
@@ -56,29 +57,38 @@ def test_engine_vs_live_cpu_reference(cuda_device, kw, ncc_tol, epe_tol, h, w, k
     assert metrics.epe_stats(got, cpu)["mean"] <= epe_tol
 
 
+def _bits_equal(got, want):
+    """got equals want bit for bit, NaN compared by position."""
+    both_nan = np.isnan(got) & np.isnan(want)
+    return bool(((got.view(np.uint32) == want.view(np.uint32)) | both_nan).all())
+
+
 @pytest.mark.parametrize("kw", [dict(), dict(flags=256), dict(fastPyramids=True), dict(polyN=7, polySigma=1.5)])
 def test_engine_matches_cuda_semantics_model(cuda_device, kw):
+    """Bit for bit against the model of the engine's roundings (oracle/farneback_model.c, build "eng")."""
     I0, I1, _ = synth.make_pair(200, 264, seed=3, kind="smooth")
     got, _ = _run(cuda_device, I0, I1, **kw)
-    ref = fm.calc(I0, I1, fm.FarnebackParams(**kw))
-    st = metrics.epe_stats(got, ref)
-    assert st["mean"] <= 1e-3 and st["p95"] <= 5e-3, st
+    P = fm.FarnebackParams(**kw)
+    ref = fn.calc(I0, I1, P, build="eng", order=fn.order_for(P))
+    assert _bits_equal(got, ref), metrics.epe_stats(got, ref)
 
 
 def test_register_blocked_iteration_matches_generic_kernel(cuda_device):
-    """kernel_path=1 forces the generic fused-iteration kernel; the K=6 register-blocked kernel
-    keeps the same summation order, so the flows agree to rounding noise."""
+    """kernel_path=1 forces the generic fused-iteration kernel (box window summed pair by pair, first gaussian tap
+    rounded on its own); the K=6 register-blocked kernel runs the tree-plus-running box sum and fuses the first gaussian
+    tap.  Each path equals the model in its own iteration order, bit for bit."""
     import torch
     import opencv_contrib_b200 as ocb
     I0, I1, _ = synth.make_pair(203, 277, seed=4, kind="smooth")
     d0, d1 = torch.from_numpy(I0).to(cuda_device), torch.from_numpy(I1).to(cuda_device)
     for flags in (0, 256):
-        outs = []
+        P = fm.FarnebackParams(flags=flags)
         for path in (0, 1):
             alg = ocb.FarnebackOpticalFlow_create(flags=flags)
             alg.setEngineOption("kernel_path", path)
-            outs.append(alg.calc(d0, d1).cpu().numpy())
-        assert float(np.abs(outs[0] - outs[1]).max()) <= 1e-4, flags
+            got = alg.calc(d0, d1).cpu().numpy()
+            ref = fn.calc(I0, I1, P, build="eng", order=fn.order_for(P, path))
+            assert _bits_equal(got, ref), (flags, path, metrics.epe_stats(got, ref))
 
 
 def test_golden_fixtures(cuda_device):
