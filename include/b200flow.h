@@ -399,13 +399,15 @@ B2F_API int b2f_calc_uv(b2f_handle *h, const b2f_image *I0, const b2f_image *I1,
  *   pos    : time position in [0,1].
  *   new_frame : device 32FC1 output, same size/step.
  *   buf    : device 32FC1 scratch of 6*rows x cols, same step, laid out like the reference's
- *            (coverage0, coverage1, fwdU, fwdV, bwdU, bwdV); zeroed by the call.
+ *            (coverage0, coverage1, fwdU, fwdV, bwdU, bwdV); the 6*rows x cols view is zeroed by the
+ *            call, the columns past cols of a pitched buf are not touched.
  *   flags  : B2F_INTERP_REFERENCE reproduces the reference bit-for-bit in formula, including its
  *            three defects (the 4th splat lands in bwdU a second time so bwdV stays 0,
  *            NPP_staging.cu:1779-1787; both samples of the "visible in both" branch read frame0,
  *            :1666; the coverage clear indexes by width not stride, :1985-1996);
- *            B2F_INTERP_CORRECTED fixes the three.  Float atomics: the sum order is not fixed,
- *            results agree to rounding (as in the reference). ---- */
+ *            B2F_INTERP_CORRECTED fixes the three.  Float atomics: the sum order of the six scratch
+ *            accumulators is not fixed, so they agree to rounding (as in the reference); the output is a
+ *            deterministic function of what the call leaves in buf. ---- */
 enum { B2F_INTERP_REFERENCE = 0, B2F_INTERP_CORRECTED = 1 };
 B2F_API int b2f_interpolate_frames(const b2f_image *frame0, const b2f_image *frame1, const b2f_image *fu,
                                    const b2f_image *fv, const b2f_image *bu, const b2f_image *bv, float pos,

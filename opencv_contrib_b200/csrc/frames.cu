@@ -183,7 +183,10 @@ extern "C" int b2f_interpolate_frames(const b2f_image *frame0, const b2f_image *
     P.bwdU = b + 4 * plane;
     P.bwdV = b + 5 * plane;
 
-    cudaError_t e = cudaMemsetAsync(b, 0, 6 * plane * sizeof(float), s);  // buf.setTo(0), :67
+    // buf.setTo(0), :67 -- the 6h x w view only: the columns past w of a pitched buf belong to the caller
+    const size_t row = (size_t)P.w * sizeof(float);
+    cudaError_t e = buf->step == row ? cudaMemsetAsync(b, 0, 6 * plane * sizeof(float), s)
+                                     : cudaMemset2DAsync(b, buf->step, 0, row, 6 * (size_t)P.h, s);
     if (e == cudaSuccess) {
         const dim3 block(32, 8), grid(div_up(P.w, 32), div_up(P.h, 8));
         k_interp_splat<<<grid, block, 0, s>>>(P, pos);

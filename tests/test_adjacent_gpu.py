@@ -1,10 +1,11 @@
 """GPU tests for the components either side of calc() (SURVEY.md 8f): planar output, interpolateFrames
-and the video front end -- all through the C ABI (ctypes).
+argument checks (its model comparisons are in test_frames_gpu.py) and the video front end -- all through the
+C ABI (ctypes).
 """
 import numpy as np
 import pytest
 
-from oracle import synth, metrics, interpolate_model as im
+from oracle import synth, metrics
 
 pytestmark = pytest.mark.gpu
 
@@ -35,51 +36,6 @@ def test_calc_uv_equals_split_of_calc(cuda_device, name):
     assert np.array_equal(u.cpu().numpy(), flow[..., 0]) and np.array_equal(v.cpu().numpy(), flow[..., 1])
     with pytest.raises(ocb.B2FError):
         alg.calcUV(d0, d1, torch.empty((90, 131, 2), device=cuda_device)[..., 0].contiguous().to(torch.float64), v0)
-
-
-@pytest.mark.parametrize("corrected", [False, True])
-@pytest.mark.parametrize("h,w,pitch", [(64, 96, 96), (75, 101, 128)])
-def test_interpolate_frames_matches_model(cuda_device, corrected, h, w, pitch):
-    import torch
-    import opencv_contrib_b200 as ocb
-    rng = np.random.default_rng(h)
-    f0 = (synth.texture(h, w, 1) / 255).astype(np.float32)
-    f1 = (synth.texture(h, w, 2) / 255).astype(np.float32)
-    fl = synth.flow_field(h, w, "smooth", seed=3)
-    bl = -synth.flow_field(h, w, "smooth", seed=3) + rng.normal(0, 0.05, (h, w, 2)).astype(np.float32)
-    planes = [f0, f1, fl[..., 0], fl[..., 1], bl[..., 0], bl[..., 1]]
-
-    def pitched(a):
-        t = torch.zeros((a.shape[0], pitch), device=cuda_device)
-        t[:, :w] = torch.from_numpy(np.ascontiguousarray(a)).to(cuda_device)
-        return t[:, :w]
-
-    d = [pitched(a) for a in planes]
-    out = pitched(np.zeros((h, w), np.float32))
-    buf = torch.full((6 * h, pitch), 7.0, device=cuda_device)[:, :w]   # must be cleared by the call
-    for pos in (0.5, 0.2):
-        got = ocb.interpolateFrames(*d, pos, out, buf, corrected=corrected)
-        torch.cuda.synchronize()
-        want, wbuf = im.interpolate_frames(*planes, pos, stride=pitch, corrected=corrected)
-        gb = buf.cpu().numpy().reshape(6, h, w)
-        # atomics: the sum order differs from the raster-order model -> rounding-level differences in the
-        # accumulators, which the division by a small coverage amplifies (twice for the reference's bwdU):
-        # compare strictly where the coverage is well away from zero
-        c0, c1 = wbuf[0, :, :w], wbuf[1, :, :w]
-        # relative to the coverage itself: where many sources converge the sums are large
-        assert (np.abs(gb[0] - c0) <= 5e-5 * np.maximum(1, c0)).all() and (np.abs(gb[1] - c1) <= 5e-5 * np.maximum(1, c1)).all()
-        well = (c0 > 0.05) & (c1 > 0.05)
-        assert well.mean() > 0.9
-        for k in range(2, 6):
-            cov = c0 if k < 4 else c1
-            ok = cov > 0.05
-            assert (np.abs(gb[k] - wbuf[k, :, :w])[ok] <= 1e-4 * (1 + np.abs(wbuf[k, :, :w][ok]))).all(), k
-            assert np.isfinite(gb[k]).all()
-        diff = np.abs(got.cpu().numpy() - want)
-        assert diff[well].max() < 2e-4, diff[well].max()
-        assert np.isfinite(got.cpu().numpy()).all()
-    if not corrected:
-        assert float(buf[5 * h:].abs().max()) == 0.0  # the reference never writes bwdV
 
 
 def test_interpolate_frames_argument_checks(cuda_device):
