@@ -185,6 +185,26 @@ typedef struct b2f_fastbm_params {
     int block_window;  /* 7  */
 } b2f_fastbm_params;
 
+/* cv::VariationalRefinement (opencv's video module, cv2.VariationalRefinement_create): the caller's flow refined in
+ * place by one calcUV call -- colour-constancy, gradient-constancy and smoothness terms, fixed-point steps of red-black
+ * SOR; the solver DeepFlow runs per level and DIS runs as its refinement stage.  Inputs 8UC1 or 32FC1 of one type and
+ * size (anything else: B2F_UNSUPPORTED_TYPE), converted to float without scaling; `flow` 32FC2 of the frame's size
+ * (b2f_calc) or two 32FC1 planes (b2f_calc_uv) is always read first and receives the result.  Every parameter value is
+ * accepted, as cv2 accepts it: an iteration count below one runs no step (the flow comes back unchanged); with
+ * epsilon 0 cv2's output turns non-finite and this engine's need not.  A flow of another type is B2F_UNSUPPORTED_TYPE,
+ * frames or a flow of another size B2F_SIZE_MISMATCH.  alpha, delta, gamma, epsilon and omega are the reference's float
+ * members: the engine rounds them to float.  The video front end refuses this engine (it has no caller flow to
+ * refine).  cv2 reports the default name "my_object"; b2f_default_name reports the same. */
+typedef struct b2f_varref_params {
+    int fixed_point_iterations; /* 5     outer (warping) iterations      */
+    int sor_iterations;         /* 5     SOR iterations per outer step   */
+    double omega;               /* 1.6   SOR relaxation                  */
+    double alpha;               /* 20    smoothness                      */
+    double delta;               /* 5     colour constancy                */
+    double gamma;               /* 10    gradient constancy              */
+    double epsilon;             /* 0.001 robust-function epsilon         */
+} b2f_varref_params;
+
 typedef struct b2f_handle b2f_handle;
 
 /* ---- construction: replaces the static ::create() factories.  A NULL params pointer means
@@ -198,6 +218,7 @@ B2F_API void b2f_denselk_default_params(b2f_denselk_params *p);
 B2F_API void b2f_deepflow_default_params(b2f_deepflow_params *p);
 B2F_API void b2f_dis_default_params(b2f_dis_params *p, int preset); /* DISOpticalFlow::create(preset) */
 B2F_API void b2f_fastbm_default_params(b2f_fastbm_params *p);
+B2F_API void b2f_varref_default_params(b2f_varref_params *p);
 
 B2F_API int b2f_tvl1_create(const b2f_tvl1_params *p, b2f_handle **out);           /* src/tvl1flow.cpp:385-391 */
 B2F_API int b2f_farneback_create(const b2f_farneback_params *p, b2f_handle **out); /* src/farneback.cpp:484-489 */
@@ -206,6 +227,7 @@ B2F_API int b2f_denselk_create(const b2f_denselk_params *p, b2f_handle **out);  
 B2F_API int b2f_deepflow_create(const b2f_deepflow_params *p, b2f_handle **out);   /* optflow deepflow.cpp:171-174 */
 B2F_API int b2f_dis_create(const b2f_dis_params *p, b2f_handle **out);             /* NULL: the FAST preset */
 B2F_API int b2f_fastbm_create(const b2f_fastbm_params *p, b2f_handle **out);       /* cudalegacy.hpp:202-211 */
+B2F_API int b2f_varref_create(const b2f_varref_params *p, b2f_handle **out);       /* VariationalRefinement::create */
 B2F_API void b2f_destroy(b2f_handle *h);
 
 /* ---- getters/setters: replace getTau()/setTau() ... (cudaoptflow.hpp:158-177,233-243,261-283,
@@ -245,6 +267,9 @@ typedef enum b2f_param_id {
     B2F_DIS_USE_MEAN_NORMALIZATION, B2F_DIS_USE_SPATIAL_PROPAGATION, B2F_DIS_USE_INITIAL_FLOW,
     /* FastOpticalFlowBM */
     B2F_FBM_SEARCH_WINDOW = 700, B2F_FBM_BLOCK_WINDOW,
+    /* VariationalRefinement: a block of its own below the active-path ids, which start at 1000 */
+    B2F_VR_FIXED_POINT_ITERATIONS = 950, B2F_VR_SOR_ITERATIONS, B2F_VR_OMEGA, B2F_VR_ALPHA, B2F_VR_DELTA, B2F_VR_GAMMA,
+    B2F_VR_EPSILON,
     /* engine knobs (no reference counterpart) */
     B2F_ENGINE_FUSED_ITERS = 900, /* TV-L1: inner iterations fused per HBM pass (0 = auto)     */
     B2F_ENGINE_USE_GRAPH = 901,   /* capture the fixed schedule in a CUDA graph (default 1)    */
@@ -281,7 +306,9 @@ typedef enum b2f_param_id {
      * solver launch per inner step; this says whether it did.  DeepFlow: the SOR iterations each solver launch of the
      * level runs (chosen from the level's shape; all of them on a level that fits one 64x64 region, which runs its
      * fixed-point steps in one launch).  DIS (s = pyramid scale, finest_scale .. coarsest): bits 0-7 the refinement's SOR
-     * iterations per solver launch (0 without refinement), bits 8-23 the patch rows hs, bits 24-39 the patch columns ws. */
+     * iterations per solver launch (0 without refinement), bits 8-23 the patch rows hs, bits 24-39 the patch columns ws.
+     * VariationalRefinement (s = 0 only): the SOR iterations each solver launch runs, as DeepFlow's; 0 when the call runs
+     * no SOR iteration. */
     B2F_ENGINE_ACTIVE_PATH = 1000
 } b2f_param_id;
 
@@ -436,8 +463,8 @@ B2F_API int b2f_calc_optical_flow_bm(const b2f_image *prev, const b2f_image *cur
 
 /* ---- batched frame-pair front end for one GPU (SURVEY.md 8b / 8e): N engine handles on N streams, pairs dealt
  *      round robin -- the pattern of the reference's own multi-stream test (test/test_optflow.cpp:468-528).
- *      algo: 1 TV-L1, 2 Farneback, 3 Brox, 4 DensePyrLK, 5 DeepFlow, 6 DIS, 7 FastOpticalFlowBM; params: the matching
- *      b2f_*_params (NULL = defaults).
+ *      algo: 1 TV-L1, 2 Farneback, 3 Brox, 4 DensePyrLK, 5 DeepFlow, 6 DIS, 7 FastOpticalFlowBM, 8 VariationalRefinement
+ *      (each pair's flow is read and refined in place); params: the matching b2f_*_params (NULL = defaults).
  *      Sharding over GPUs / processes and the NCCL result gather stay with the caller's process framework
  *      (opencv_contrib_b200/batch.py over torch.distributed). ---- */
 typedef struct b2f_batch b2f_batch;
@@ -486,7 +513,9 @@ B2F_API void b2f_batch_destroy(b2f_batch *b);
  *      no host synchronisation inside push), and with `warm_start` the previous pair's flow seeds
  *      the next solve (tvl1flow.cpp:203-207,249-256 useInitialFlow; farneback.cpp:179-188,398-404
  *      OPTFLOW_USE_INITIAL_FLOW; the temporal chaining the reference's test does by hand,
- *      test_optflow.cpp:328-334).  `depth` = pairs in flight (ring of host-visible results). ---- */
+ *      test_optflow.cpp:328-334).  `depth` = pairs in flight (ring of host-visible results).  A
+ *      VariationalRefinement handle is refused with B2F_BAD_ARG: it refines a caller's flow, which the frame loop does
+ *      not have, and the loop reuses its flow slots. ---- */
 typedef struct b2f_video b2f_video;
 B2F_API int b2f_video_create(b2f_handle *h, int rows, int cols, int type, int depth, int warm_start,
                              b2f_video **out);

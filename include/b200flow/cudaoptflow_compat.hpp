@@ -325,6 +325,45 @@ public:
     }
 };
 
+/** cv::VariationalRefinement (opencv's video module) on the GPU, with its accessors, in the cv::cuda calling convention:
+ *  calc refines `flow` (32FC2 of the frame's size, always read) in place, calcUV the same on two 32FC1 planes.  u8 or
+ *  float images, used without scaling (see b2f_varref_params). */
+class VariationalRefinement : public DenseOpticalFlow, protected impl::HandleOwner {
+public:
+    B2F_ACCESSOR(int, FixedPointIterations, B2F_VR_FIXED_POINT_ITERATIONS)
+    B2F_ACCESSOR(int, SorIterations, B2F_VR_SOR_ITERATIONS)
+    B2F_ACCESSOR(float, Omega, B2F_VR_OMEGA)
+    B2F_ACCESSOR(float, Alpha, B2F_VR_ALPHA)
+    B2F_ACCESSOR(float, Delta, B2F_VR_DELTA)
+    B2F_ACCESSOR(float, Gamma, B2F_VR_GAMMA)
+    B2F_ACCESSOR(float, Epsilon, B2F_VR_EPSILON)
+
+    void calc(InputArray I0, InputArray I1, InputOutputArray flow, Stream &stream = Stream::Null()) override {
+        run(I0, I1, flow, stream, true);
+    }
+    void calcUV(InputArray I0, InputArray I1, InputOutputArray flow_u, InputOutputArray flow_v,
+                Stream &stream = Stream::Null()) {
+        const auto &a = detail::in_mat(I0);
+        const auto &b = detail::in_mat(I1);
+        auto &u = detail::out_ref(flow_u);
+        auto &v = detail::out_ref(flow_v);
+        b2f_image i0{a.data, a.step, a.rows, a.cols, a.type()};
+        b2f_image i1{b.data, b.step, b.rows, b.cols, b.type()};
+        b2f_image iu{u.data, u.step, u.rows, u.cols, u.type()};
+        b2f_image iv{v.data, v.step, v.rows, v.cols, v.type()};
+        const int st = b2f_calc_uv(h_, &i0, &i1, &iu, &iv, detail::raw(stream));
+        if (st != B2F_OK) detail::fail(st, "VariationalRefinement::calcUV");
+    }
+    String getDefaultName() const override { return b2f_default_name(h_); }
+
+    static Ptr<VariationalRefinement> create() {
+        auto o = detail::make<VariationalRefinement>();
+        const int st = b2f_varref_create(nullptr, &o->h_);
+        if (st != B2F_OK) detail::fail(st, "VariationalRefinement::create");
+        return o;
+    }
+};
+
 /** cv::cuda::FastOpticalFlowBM (cudalegacy.hpp:202-211): operator() with the reference's signature; flowx / flowy are
  *  (re)allocated as CV_32FC1 of the frame's size.  Also a DenseOpticalFlow (calc writes CV_32FC2 with the handle's
  *  windows).  Refused windows: see b2f_fastbm_params. */

@@ -21,12 +21,14 @@ from .cudaoptflow import (  # noqa: F401
     DensePyrLKOpticalFlow,
     DeepFlowOpticalFlow,
     DISOpticalFlow,
+    VariationalRefinement,
     OpticalFlowDual_TVL1_create,
     FarnebackOpticalFlow_create,
     BroxOpticalFlow_create,
     DensePyrLKOpticalFlow_create,
     createOptFlow_DeepFlow,
     DISOpticalFlow_create,
+    VariationalRefinement_create,
     DISOPTICAL_FLOW_PRESET_ULTRAFAST,
     DISOPTICAL_FLOW_PRESET_FAST,
     DISOPTICAL_FLOW_PRESET_MEDIUM,

@@ -67,6 +67,11 @@ class b2f_fastbm_params(C.Structure):
     _fields_ = [("search_window", C.c_int), ("block_window", C.c_int)]
 
 
+class b2f_varref_params(C.Structure):
+    _fields_ = [("fixed_point_iterations", C.c_int), ("sor_iterations", C.c_int), ("omega", C.c_double),
+                ("alpha", C.c_double), ("delta", C.c_double), ("gamma", C.c_double), ("epsilon", C.c_double)]
+
+
 class b2f_sparselk_params(C.Structure):
     _fields_ = [("win_width", C.c_int), ("win_height", C.c_int), ("max_level", C.c_int), ("iters", C.c_int),
                 ("use_initial_flow", C.c_int)]
@@ -121,6 +126,8 @@ SYMBOLS = [
     ("b2f_dis_create", C.c_int, [C.POINTER(b2f_dis_params), C.POINTER(_H)]),
     ("b2f_fastbm_default_params", None, [C.POINTER(b2f_fastbm_params)]),
     ("b2f_fastbm_create", C.c_int, [C.POINTER(b2f_fastbm_params), C.POINTER(_H)]),
+    ("b2f_varref_default_params", None, [C.POINTER(b2f_varref_params)]),
+    ("b2f_varref_create", C.c_int, [C.POINTER(b2f_varref_params), C.POINTER(_H)]),
     ("b2f_calc_optical_flow_bm_size", C.c_int, [C.c_int] * 8 + [C.POINTER(C.c_int)] * 3),
     ("b2f_calc_optical_flow_bm", C.c_int, [_IMG, _IMG] + [C.c_int] * 7 + [_IMG, _IMG, C.c_void_p]),
     ("b2f_destroy", None, [_H]),
@@ -227,6 +234,8 @@ PARAM = {
                 variational_refinement_iterations=605, alpha=606, delta=607, gamma=608, epsilon=609,
                 use_mean_normalization=610, use_spatial_propagation=611, use_initial_flow=612),
     "fastbm": dict(search_window=700, block_window=701),
+    "varref": dict(fixed_point_iterations=950, sor_iterations=951, omega=952, alpha=953, delta=954, gamma=955,
+                   epsilon=956),
     "superres": dict(scale=800, iterations=801, tau=802, lambda_=803, alpha=804, btv_kernel_size=805,
                      blur_kernel_size=806, blur_sigma=807, temporal_area_radius=808),
     "engine": dict(fused_iters=900, use_graph=901, kernel_path=902, aux_path=903, active_path=1000),

@@ -80,6 +80,8 @@ void b2f_video_destroy(b2f_video *v) {
 int b2f_video_create(b2f_handle *h, int rows, int cols, int type, int depth, int warm_start, b2f_video **out) {
     if (!h || !out || rows <= 0 || cols <= 0 || depth < 1 || depth > 64) return B2F_BAD_ARG;
     if (type != B2F_8UC1 && type != B2F_32FC1) return B2F_UNSUPPORTED_TYPE;
+    // VariationalRefinement refines the caller's flow: the frame loop has none, and it reuses its flow slots
+    if (h->algo == b2f::ALGO_VARREF) return B2F_BAD_ARG;
     *out = nullptr;
     b2f_video *v = new b2f_video;
     v->h = h;

@@ -312,6 +312,25 @@ _accessors(DISOpticalFlow, "dis", {
 DISOPTICAL_FLOW_PRESET_ULTRAFAST, DISOPTICAL_FLOW_PRESET_FAST, DISOPTICAL_FLOW_PRESET_MEDIUM = 0, 1, 2
 
 
+class VariationalRefinement(DenseOpticalFlow):
+    """cv::VariationalRefinement (opencv's video module) on the GPU, with cv2's accessor names: ``calc(I0, I1, flow)``
+    refines ``flow`` in place and returns it, ``calcUV(I0, I1, u, v)`` does the same on planes.  The flow is always
+    read, so it must be given.  Inputs are u8 or float32, used without scaling."""
+
+    def _needs_initial_flow(self) -> bool:
+        return True
+
+    def getActivePath(self) -> int:
+        """SOR iterations per solver launch the last calc ran (B2F_ENGINE_ACTIVE_PATH); 0 when it ran none."""
+        return int(self._get(PARAM["engine"]["active_path"]))
+
+
+_accessors(VariationalRefinement, "varref", {
+    "fixed_point_iterations": ("FixedPointIterations", int), "sor_iterations": ("SorIterations", int),
+    "omega": ("Omega", float), "alpha": ("Alpha", float), "delta": ("Delta", float), "gamma": ("Gamma", float),
+    "epsilon": ("Epsilon", float)})
+
+
 def _create(cls, fn_name: str, params):
     l = _lib.lib()
     h = C.c_void_p()
@@ -364,6 +383,13 @@ def DISOpticalFlow_create(preset=DISOPTICAL_FLOW_PRESET_FAST):
     p = _lib.b2f_dis_params()
     _lib.lib().b2f_dis_default_params(C.byref(p), int(preset))
     return _create(DISOpticalFlow, "b2f_dis_create", p)
+
+
+def VariationalRefinement_create():
+    """cv::VariationalRefinement::create() (cv2.VariationalRefinement_create), with the reference's defaults."""
+    p = _lib.b2f_varref_params()
+    _lib.lib().b2f_varref_default_params(C.byref(p))
+    return _create(VariationalRefinement, "b2f_varref_create", p)
 
 
 class FastOpticalFlowBM(DenseOpticalFlow):
