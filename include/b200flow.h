@@ -712,6 +712,61 @@ B2F_API int b2f_gftt_last_info(b2f_corners *h, b2f_gftt_info *out, void *cuda_st
 B2F_API int b2f_corners_last_cuda_error(const b2f_corners *h);
 B2F_API void b2f_corners_destroy(b2f_corners *h);
 
+/* ---- the video module's pyramidal Lucas-Kanade tracker: cv::buildOpticalFlowPyramid, cv::calcOpticalFlowPyrLK and
+ *      cv::SparsePyrLKOpticalFlow (video/tracking.hpp), bit for bit equal to cv2 4.13's x86 build, including the order in
+ *      which it adds its float sums (DESIGN §4.13).  This is a second tracker next to b2f_sparselk_* (cv::cuda semantics).
+ *   Frames: device 8U with 1 to 256 interleaved channels (another depth: B2F_UNSUPPORTED_TYPE), pitched or an ROI.
+ *   Pyramids (b2f_lkpyr_pyramid): device levels with a (win_w, win_h) border, BORDER_REFLECT_101 for the uint8 levels
+ *      and BORDER_CONSTANT for the int16 Scharr derivatives (CV_16SC(2 cn), Ix and Iy per channel); other border modes
+ *      are refused with B2F_UNSUPPORTED_TYPE (BORDER_ISOLATED is accepted and implied).  A pyramid grows on demand; a
+ *      build that needs more memory first waits for its stream.  b2f_lkpyr_pyramid_level views a level, border
+ *      included: rows + 2 win_h by cols + 2 win_w.
+ *   b2f_lkpyr_calc: prev and next are each an image or a pyramid (exactly one of the two pointers).  A pyramid caps
+ *      max_level at its own level count and must have a border of at least the window (else B2F_BAD_ARG); an image is
+ *      built up to what is left.  prev_pts / next_pts: n_points interleaved (x, y) float32 on the device; status: n
+ *      bytes; err: n float32 or NULL.  next_pts is read first only with B2F_LKPYR_USE_INITIAL_FLOW.  err is written where
+ *      cv2 writes it (tracked points, points outside the image on level 0 (0), and every point that reached the
+ *      covariance under B2F_LKPYR_GET_MIN_EIGENVALS); elsewhere the caller's values stay.  Everything runs on
+ *      `cuda_stream` without host synchronisation (a NULL stream ends with a device synchronise); the first call at a
+ *      new size waits for the stream while it lays out the handle's workspace.  A handle may be called on several
+ *      streams: a call on another stream than the previous call first waits (on the device) for that call's work,
+ *      since both share the handle's workspace.  A pyramid is the caller's memory: rebuilding it while a calc on
+ *      another stream still reads it is the caller's race, and a rebuild at another size, channel count, window,
+ *      level count or derivative choice moves its levels, so views taken before it are stale. ---- */
+enum { B2F_LKPYR_USE_INITIAL_FLOW = 4, B2F_LKPYR_GET_MIN_EIGENVALS = 8 }; /* cv::OPTFLOW_USE_INITIAL_FLOW, OPTFLOW_LK_GET_MIN_EIGENVALS */
+typedef struct b2f_lkpyr_params {
+    int win_width;            /* 21 */
+    int win_height;           /* 21 */
+    int max_level;            /* 3  */
+    int criteria_type;        /* 3: TermCriteria::COUNT (1) | TermCriteria::EPS (2) */
+    int max_count;            /* 30 */
+    double epsilon;           /* 0.01 */
+    int flags;                /* 0  */
+    double min_eig_threshold; /* 1e-4 */
+} b2f_lkpyr_params;
+typedef struct b2f_lkpyr b2f_lkpyr;
+typedef struct b2f_lkpyr_pyramid b2f_lkpyr_pyramid;
+B2F_API void b2f_lkpyr_default_params(b2f_lkpyr_params *p);
+B2F_API int b2f_lkpyr_create(const b2f_lkpyr_params *p, b2f_lkpyr **out); /* NULL: the defaults */
+B2F_API int b2f_lkpyr_set_params(b2f_lkpyr *h, const b2f_lkpyr_params *p);
+B2F_API int b2f_lkpyr_get_params(const b2f_lkpyr *h, b2f_lkpyr_params *p);
+/* borrowed base handle, for b2f_get_param(B2F_ENGINE_ACTIVE_PATH) and b2f_get_stats */
+B2F_API b2f_handle *b2f_lkpyr_engine(b2f_lkpyr *h);
+B2F_API int b2f_lkpyr_pyramid_create(b2f_lkpyr_pyramid **out);
+B2F_API void b2f_lkpyr_pyramid_destroy(b2f_lkpyr_pyramid *p);
+/* buildOpticalFlowPyramid: *max_level_out receives its return value (the last level built) */
+B2F_API int b2f_lkpyr_build_pyramid(const b2f_image *img, int win_w, int win_h, int max_level, int with_derivatives,
+                                    int pyr_border, int deriv_border, b2f_lkpyr_pyramid *pyr, int *max_level_out,
+                                    void *cuda_stream);
+B2F_API int b2f_lkpyr_pyramid_info(const b2f_lkpyr_pyramid *p, int *levels, int *win_w, int *win_h,
+                                   int *with_derivatives);
+B2F_API int b2f_lkpyr_pyramid_level(const b2f_lkpyr_pyramid *p, int level, int deriv, b2f_image *view);
+B2F_API int b2f_lkpyr_calc(b2f_lkpyr *h, const b2f_image *prev_img, const b2f_lkpyr_pyramid *prev_pyr,
+                           const b2f_image *next_img, const b2f_lkpyr_pyramid *next_pyr, const float *prev_pts,
+                           float *next_pts, unsigned char *status, float *err, int n_points, void *cuda_stream);
+B2F_API int b2f_lkpyr_last_cuda_error(const b2f_lkpyr *h);
+B2F_API void b2f_lkpyr_destroy(b2f_lkpyr *h);
+
 #ifdef __cplusplus
 }
 #endif

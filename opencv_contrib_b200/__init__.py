@@ -12,6 +12,7 @@ Only what the hot path needs lives here:
   flowio.py        Middlebury .flo files + the reference's error statistics
   superres.py      superres's BTV-L1 video super-resolution and its four CUDA optical-flow wrappers
   cudaimgproc.py   cudaimgproc's corner responses and GoodFeaturesToTrack detector
+  lkpyramid.py     the video module's calcOpticalFlowPyrLK, buildOpticalFlowPyramid and SparsePyrLKOpticalFlow
 """
 from .cudaoptflow import (  # noqa: F401
     DenseOpticalFlow,
@@ -57,3 +58,4 @@ from .cudaimgproc import (  # noqa: F401
     createMinEigenValCorner,
     createGoodFeaturesToTrackDetector,
 )
+from .lkpyramid import buildOpticalFlowPyramid, calcOpticalFlowPyrLK  # noqa: F401

@@ -92,6 +92,11 @@ class b2f_gftt_info(C.Structure):
     _fields_ = [("candidates", C.c_int), ("kept", C.c_int), ("capped", C.c_int), ("rounds", C.c_int)]
 
 
+class b2f_lkpyr_params(C.Structure):
+    _fields_ = [("win_width", C.c_int), ("win_height", C.c_int), ("max_level", C.c_int), ("criteria_type", C.c_int),
+                ("max_count", C.c_int), ("epsilon", C.c_double), ("flags", C.c_int), ("min_eig_threshold", C.c_double)]
+
+
 class b2f_stats(C.Structure):
     _fields_ = [("calls", C.c_uint64), ("launches", C.c_uint64),
                 ("class_launches", C.c_uint64 * B2F_MAX_KERNEL_CLASSES),
@@ -207,6 +212,21 @@ SYMBOLS = [
     ("b2f_gftt_last_info", C.c_int, [_H, C.POINTER(b2f_gftt_info), C.c_void_p]),
     ("b2f_corners_last_cuda_error", C.c_int, [_H]),
     ("b2f_corners_destroy", None, [_H]),
+    ("b2f_lkpyr_default_params", None, [C.POINTER(b2f_lkpyr_params)]),
+    ("b2f_lkpyr_create", C.c_int, [C.POINTER(b2f_lkpyr_params), C.POINTER(_H)]),
+    ("b2f_lkpyr_set_params", C.c_int, [_H, C.POINTER(b2f_lkpyr_params)]),
+    ("b2f_lkpyr_get_params", C.c_int, [_H, C.POINTER(b2f_lkpyr_params)]),
+    ("b2f_lkpyr_engine", C.c_void_p, [_H]),
+    ("b2f_lkpyr_pyramid_create", C.c_int, [C.POINTER(_H)]),
+    ("b2f_lkpyr_pyramid_destroy", None, [_H]),
+    ("b2f_lkpyr_build_pyramid", C.c_int, [_IMG, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, _H,
+                                          C.POINTER(C.c_int), C.c_void_p]),
+    ("b2f_lkpyr_pyramid_info", C.c_int, [_H] + [C.POINTER(C.c_int)] * 4),
+    ("b2f_lkpyr_pyramid_level", C.c_int, [_H, C.c_int, C.c_int, _IMG]),
+    ("b2f_lkpyr_calc", C.c_int, [_H, _IMG, _H, _IMG, _H, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int,
+                                 C.c_void_p]),
+    ("b2f_lkpyr_last_cuda_error", C.c_int, [_H]),
+    ("b2f_lkpyr_destroy", None, [_H]),
     ("b2f_flo_read_size", C.c_int, [C.c_char_p, C.POINTER(C.c_int), C.POINTER(C.c_int)]),
     ("b2f_flo_read", C.c_int, [C.c_char_p, C.c_void_p, C.c_size_t, C.c_int, C.c_int]),
     ("b2f_flo_write", C.c_int, [C.c_char_p, C.c_void_p, C.c_size_t, C.c_int, C.c_int]),
