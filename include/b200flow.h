@@ -205,6 +205,25 @@ typedef struct b2f_varref_params {
     double epsilon;             /* 0.001 robust-function epsilon         */
 } b2f_varref_params;
 
+/* cv::calcOpticalFlowFarneback / cv::FarnebackOpticalFlow (opencv's video module, modules/video/src/optflowgf.cpp), bit
+ * for bit equal to cv2 4.x's portable CPU path (cv2.setUseOptimized(False) with IPP off, the SSE baseline code every
+ * x86-64 host runs; DESIGN §4.14).  Created by b2f_optflowgf_create from a b2f_farneback_params, whose fields are the
+ * video class's create() arguments, and driven by the B2F_FARN_* parameter ids.  Unlike b2f_farneback_create (the
+ * cv::cuda class) it follows the CPU class: centre-aligned level images blurred from the full-size frame, double box
+ * sums, fastPyramids accepted and ignored.  Frames 8UC1 or 32FC1 of one type and size (cv2 also takes other depths:
+ * here they are B2F_UNSUPPORTED_TYPE); the flow 32FC2 (b2f_calc) or two 32FC1 planes (b2f_calc_uv), read first with
+ * B2F_OPTFLOW_USE_INITIAL_FLOW.  B2F_BAD_ARG: pyr_scale >= 1 (cv2 asserts), poly_n outside 1..B2F_OPTFLOWGF_MAX_POLY_N,
+ * win_size outside 1..B2F_OPTFLOWGF_MAX_WIN_SIZE, or a deepest-level blur wider than 255 taps.  That blur has
+ * ksize = max(cvRound(2.5 (1/scale - 1)) | 1, 3) at the deepest level's scale, so it is refused once 1/scale reaches about
+ * 103: at pyr_scale 0.5 with num_levels >= 7 and a shorter side of at least 4096 (1/scale 128, ksize 319); never with the
+ * default 5 levels.  A handle may be called on several streams: a call on another stream than the previous call waits
+ * for it, since both use the handle's workspace.  b2f_default_name reports "DenseOpticalFlow.FarnebackOpticalFlow", as
+ * cv2 does. */
+enum { B2F_OPTFLOWGF_MAX_POLY_N = 15, B2F_OPTFLOWGF_MAX_WIN_SIZE = 255 };
+/* B2F_ENGINE_ACTIVE_PATH + level (finest first) of an optflowgf handle: the window the level ran, plus AREA_LEVEL when
+ * its images came through OpenCV's exact-half fast INTER_AREA rule */
+enum { B2F_OPTFLOWGF_PATH_BOX = 1, B2F_OPTFLOWGF_PATH_GAUSSIAN = 2, B2F_OPTFLOWGF_PATH_AREA_LEVEL = 4 };
+
 typedef struct b2f_handle b2f_handle;
 
 /* ---- construction: replaces the static ::create() factories.  A NULL params pointer means
@@ -228,6 +247,7 @@ B2F_API int b2f_deepflow_create(const b2f_deepflow_params *p, b2f_handle **out);
 B2F_API int b2f_dis_create(const b2f_dis_params *p, b2f_handle **out);             /* NULL: the FAST preset */
 B2F_API int b2f_fastbm_create(const b2f_fastbm_params *p, b2f_handle **out);       /* cudalegacy.hpp:202-211 */
 B2F_API int b2f_varref_create(const b2f_varref_params *p, b2f_handle **out);       /* VariationalRefinement::create */
+B2F_API int b2f_optflowgf_create(const b2f_farneback_params *p, b2f_handle **out); /* video FarnebackOpticalFlow */
 B2F_API void b2f_destroy(b2f_handle *h);
 
 /* ---- getters/setters: replace getTau()/setTau() ... (cudaoptflow.hpp:158-177,233-243,261-283,
@@ -464,7 +484,8 @@ B2F_API int b2f_calc_optical_flow_bm(const b2f_image *prev, const b2f_image *cur
 /* ---- batched frame-pair front end for one GPU (SURVEY.md 8b / 8e): N engine handles on N streams, pairs dealt
  *      round robin -- the pattern of the reference's own multi-stream test (test/test_optflow.cpp:468-528).
  *      algo: 1 TV-L1, 2 Farneback, 3 Brox, 4 DensePyrLK, 5 DeepFlow, 6 DIS, 7 FastOpticalFlowBM, 8 VariationalRefinement
- *      (each pair's flow is read and refined in place); params: the matching b2f_*_params (NULL = defaults).
+ *      (each pair's flow is read and refined in place), 9 the video module's Farneback (b2f_optflowgf_create; params a
+ *      b2f_farneback_params); params: the matching b2f_*_params (NULL = defaults).
  *      Sharding over GPUs / processes and the NCCL result gather stay with the caller's process framework
  *      (opencv_contrib_b200/batch.py over torch.distributed). ---- */
 typedef struct b2f_batch b2f_batch;

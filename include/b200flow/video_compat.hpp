@@ -6,7 +6,10 @@
 // b200flow, as cv:: holds them next to cv::cuda::, and work on device memory: frames are 8U GpuMats (or an
 // OpticalFlowPyramid built from one), points 1 x N CV_32FC2 GpuMats, status 1 x N CV_8UC1 and err 1 x N CV_32FC1.
 // Results equal cv::calcOpticalFlowPyrLK bit for bit; b200flow::cuda::SparsePyrLKOpticalFlow is the cv::cuda tracker.
+// The video module's Farneback flow (calcOpticalFlowFarneback, FarnebackOpticalFlow; b2f_optflowgf_*) is here too.
 #pragma once
+
+#include <map>
 
 #include "cudaoptflow_compat.hpp"
 
@@ -156,6 +159,63 @@ inline void calcOpticalFlowPyrLK(LkFrame prevImg, LkFrame nextImg, const GpuMat 
                                  int flags = 0, double minEigThreshold = 1e-4, Stream &stream = Stream::Null()) {
     SparsePyrLKOpticalFlow lk(winSize, maxLevel, criteria, flags, minEigThreshold);
     lk.calc(prevImg, nextImg, prevPts, nextPts, status, err, stream);
+}
+
+/** cv::FarnebackOpticalFlow (the video module's class; b2f_optflowgf_create): results equal cv2's portable CPU path bit
+ * for bit.  b200flow::cuda::FarnebackOpticalFlow is the cv::cuda class. */
+#define B2F_GF_ACCESSOR(T, Name, ID)                        \
+    T get##Name() const { return static_cast<T>(get(ID)); } \
+    void set##Name(T v) { set(ID, static_cast<double>(v)); }
+
+class FarnebackOpticalFlow : public cuda::DenseOpticalFlow, protected cuda::impl::HandleOwner {
+public:
+    B2F_GF_ACCESSOR(int, NumLevels, B2F_FARN_NUM_LEVELS)
+    B2F_GF_ACCESSOR(double, PyrScale, B2F_FARN_PYR_SCALE)
+    B2F_GF_ACCESSOR(bool, FastPyramids, B2F_FARN_FAST_PYRAMIDS)
+    B2F_GF_ACCESSOR(int, WinSize, B2F_FARN_WIN_SIZE)
+    B2F_GF_ACCESSOR(int, NumIters, B2F_FARN_NUM_ITERS)
+    B2F_GF_ACCESSOR(int, PolyN, B2F_FARN_POLY_N)
+    B2F_GF_ACCESSOR(double, PolySigma, B2F_FARN_POLY_SIGMA)
+    B2F_GF_ACCESSOR(int, Flags, B2F_FARN_FLAGS)
+
+    void calc(cuda::InputArray I0, cuda::InputArray I1, cuda::InputOutputArray flow,
+              Stream &stream = Stream::Null()) override {
+        run(I0, I1, flow, stream, (getFlags() & cuda::OPTFLOW_USE_INITIAL_FLOW) != 0);
+    }
+    cuda::String getDefaultName() const override { return b2f_default_name(h_); }
+
+    static Ptr<FarnebackOpticalFlow> create(int numLevels = 5, double pyrScale = 0.5, bool fastPyramids = false,
+                                            int winSize = 13, int numIters = 10, int polyN = 5,
+                                            double polySigma = 1.1, int flags = 0) {
+        b2f_farneback_params p{numLevels, pyrScale, fastPyramids, winSize, numIters, polyN, polySigma, flags};
+        auto o = detail::make<FarnebackOpticalFlow>();
+        const int st = b2f_optflowgf_create(&p, &o->h_);
+        if (st != B2F_OK) detail::fail(st, "FarnebackOpticalFlow::create");
+        return o;
+    }
+};
+
+#undef B2F_GF_ACCESSOR
+
+/** cv::calcOpticalFlowFarneback, on one handle per host thread and device whose workspace persists between calls.
+ * Calls on different streams are safe: the handle orders a call on another stream after the previous call. */
+inline void calcOpticalFlowFarneback(const GpuMat &prev, const GpuMat &next, GpuMat &flow, double pyr_scale, int levels,
+                                     int winsize, int iterations, int poly_n, double poly_sigma, int flags,
+                                     Stream &stream = Stream::Null()) {
+    // a handle belongs to the device of its first call
+    thread_local std::map<int, Ptr<FarnebackOpticalFlow>> handles;
+    int dev = 0;
+    if (cudaGetDevice(&dev) != cudaSuccess) detail::fail(B2F_NO_DEVICE, "calcOpticalFlowFarneback");
+    Ptr<FarnebackOpticalFlow> &fb = handles[dev];
+    if (!fb) fb = FarnebackOpticalFlow::create();
+    fb->setPyrScale(pyr_scale);
+    fb->setNumLevels(levels);
+    fb->setWinSize(winsize);
+    fb->setNumIters(iterations);
+    fb->setPolyN(poly_n);
+    fb->setPolySigma(poly_sigma);
+    fb->setFlags(flags);
+    fb->calc(prev, next, flow, stream);
 }
 
 }  // namespace b200flow

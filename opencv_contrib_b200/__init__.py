@@ -13,6 +13,7 @@ Only what the hot path needs lives here:
   superres.py      superres's BTV-L1 video super-resolution and its four CUDA optical-flow wrappers
   cudaimgproc.py   cudaimgproc's corner responses and GoodFeaturesToTrack detector
   lkpyramid.py     the video module's calcOpticalFlowPyrLK, buildOpticalFlowPyramid and SparsePyrLKOpticalFlow
+  optflowgf.py     the video module's calcOpticalFlowFarneback and FarnebackOpticalFlow
 """
 from .cudaoptflow import (  # noqa: F401
     DenseOpticalFlow,
@@ -59,3 +60,5 @@ from .cudaimgproc import (  # noqa: F401
     createGoodFeaturesToTrackDetector,
 )
 from .lkpyramid import buildOpticalFlowPyramid, calcOpticalFlowPyrLK  # noqa: F401
+from . import optflowgf  # noqa: F401
+from .optflowgf import calcOpticalFlowFarneback  # noqa: F401

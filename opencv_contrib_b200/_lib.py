@@ -133,6 +133,7 @@ SYMBOLS = [
     ("b2f_fastbm_create", C.c_int, [C.POINTER(b2f_fastbm_params), C.POINTER(_H)]),
     ("b2f_varref_default_params", None, [C.POINTER(b2f_varref_params)]),
     ("b2f_varref_create", C.c_int, [C.POINTER(b2f_varref_params), C.POINTER(_H)]),
+    ("b2f_optflowgf_create", C.c_int, [C.POINTER(b2f_farneback_params), C.POINTER(_H)]),
     ("b2f_calc_optical_flow_bm_size", C.c_int, [C.c_int] * 8 + [C.POINTER(C.c_int)] * 3),
     ("b2f_calc_optical_flow_bm", C.c_int, [_IMG, _IMG] + [C.c_int] * 7 + [_IMG, _IMG, C.c_void_p]),
     ("b2f_destroy", None, [_H]),

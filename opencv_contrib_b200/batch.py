@@ -97,7 +97,8 @@ class NativeFlowBatch:
         NativeFlowBatch("tvl1", dict(nscales=5, warps=10, epsilon=0.0, iterations=30), n_streams=4)
     """
 
-    _ALGO = {"tvl1": 1, "farneback": 2, "brox": 3, "denselk": 4, "deepflow": 5, "dis": 6, "fastbm": 7, "varref": 8}
+    _ALGO = {"tvl1": 1, "farneback": 2, "brox": 3, "denselk": 4, "deepflow": 5, "dis": 6, "fastbm": 7, "varref": 8,
+             "optflowgf": 9}
 
     def __init__(self, family: str, params: dict | None = None, n_streams: int = 4):
         import ctypes as C
@@ -107,9 +108,11 @@ class NativeFlowBatch:
         struct = {"tvl1": _lib.b2f_tvl1_params, "farneback": _lib.b2f_farneback_params, "brox": _lib.b2f_brox_params,
                   "denselk": _lib.b2f_denselk_params, "deepflow": _lib.b2f_deepflow_params,
                   "dis": _lib.b2f_dis_params, "fastbm": _lib.b2f_fastbm_params,
-                  "varref": _lib.b2f_varref_params}[family]()
+                  "varref": _lib.b2f_varref_params, "optflowgf": _lib.b2f_farneback_params}[family]()
         preset = (1,) if family == "dis" else ()  # DIS defaults: the FAST preset
-        getattr(self._lib, "b2f_%s_default_params" % family)(C.byref(struct), *preset)
+        # the video module's Farneback takes the cv::cuda class's parameter struct and defaults
+        defaults = "farneback" if family == "optflowgf" else family
+        getattr(self._lib, "b2f_%s_default_params" % defaults)(C.byref(struct), *preset)
         for k, v in (params or {}).items():
             if not hasattr(struct, k):
                 raise AttributeError("%s has no parameter %r" % (family, k))

@@ -108,6 +108,7 @@ int b2f_batch_create(int algo, const void *params, int n_streams, b2f_batch **ou
             case b2f::ALGO_DIS: st = b2f_dis_create(static_cast<const b2f_dis_params *>(params), &h); break;
             case b2f::ALGO_FASTBM: st = b2f_fastbm_create(static_cast<const b2f_fastbm_params *>(params), &h); break;
             case b2f::ALGO_VARREF: st = b2f_varref_create(static_cast<const b2f_varref_params *>(params), &h); break;
+            case b2f::ALGO_OPTFLOWGF: st = b2f_optflowgf_create(static_cast<const b2f_farneback_params *>(params), &h); break;
             default: st = B2F_BAD_ARG;
         }
         if (st != B2F_OK) break;

@@ -148,7 +148,7 @@ private:
 // Handle base
 // ---------------------------------------------------------------------------------------------
 enum Algo { ALGO_TVL1 = 1, ALGO_FARNEBACK = 2, ALGO_BROX = 3, ALGO_DENSELK = 4, ALGO_DEEPFLOW = 5, ALGO_DIS = 6, ALGO_FASTBM = 7,
-           ALGO_VARREF = 8 };
+           ALGO_VARREF = 8, ALGO_OPTFLOWGF = 9 };
 
 struct EngineKnobs {
     int fused_iters = 0;  // 0 = auto

@@ -96,7 +96,7 @@ int b2f_video_create(b2f_handle *h, int rows, int cols, int type, int depth, int
             v->warm_param = B2F_TVL1_USE_INITIAL_FLOW;
             v->warm_on = 1;
             v->warm_off = 0;
-        } else if (h->algo == b2f::ALGO_FARNEBACK) {
+        } else if (h->algo == b2f::ALGO_FARNEBACK || h->algo == b2f::ALGO_OPTFLOWGF) {
             double flags = 0;
             b2f_get_param(h, B2F_FARN_FLAGS, &flags);
             v->warm_param = B2F_FARN_FLAGS;
